@@ -104,7 +104,7 @@ struct KSubHist {  // one BasicHist bucket layout (hist_basic.go:34-70)
 
 struct KAgg {
   int32_t col;
-  int32_t nsub;  // 0: no buckets (avg mode); 1: BasicHist; >1: MultiHist subhists
+  int32_t nsub;  // number of bucket layouts: 0 in avg mode, 1 for a BasicHist, the sub-ranges of a MultiHist
   int64_t info_min, info_max;
   int64_t reject_hi;
   uint32_t nvals_total;
@@ -112,7 +112,7 @@ struct KAgg {
                       // kernel then skips the hist-Count reductions; accumulators-in-global plans only)
   uint32_t hrow_off;  // offset of this aggregation's counters inside a slot's row of the shared-memory
                       // histogram cache (HROW_NONE: its buckets go straight to L2)
-  uint32_t _pad2;
+  uint32_t multi;     // a MultiHist: a value outside every sub-range takes no bucket (also with one sub-range)
   uint64_t* buckets;  // [nslots][nvals_total]
   uint64_t* hcount;   // [nslots]
   uint64_t* sum;      // [nslots]

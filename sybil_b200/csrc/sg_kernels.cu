@@ -1197,7 +1197,7 @@ __device__ __forceinline__ uint32_t time_code(long long v, long long bucket, lon
 // ---------------------------------------------------------------------------
 struct AggSlow {  // what the out-of-line paths need (lives in local memory)
   long long info_min, info_max, reject_hi;
-  int nsub;
+  int nsub, multi;
   uint32_t nvals_total;
   unsigned long long* buckets;
   unsigned long long* hcount;
@@ -1205,10 +1205,9 @@ struct AggSlow {  // what the out-of-line paths need (lives in local memory)
   long long* vmax;
   const KSubHist* sub;
   uint32_t acc_w0_s;  // shared address of word0 of this aggregation for slot 0, this lane's replica
-  uint32_t hi_s;      // shared address of the (unreplicated) sum high limb of this aggregation for slot 0
-  uint32_t hi_stride_b;  // bytes between two slots' high limbs
+  unsigned long long* csum;  // this aggregation's sum in the CTA's 64-bit totals (shared memory), slot 0
+  uint32_t ctw;              // words per slot of those totals
   uint32_t gstride_b;  // bytes between two slots' accumulators
-  uint32_t R_b;        // bytes between two words' replicas
   int acc_smem;
   uint32_t tb;         // global slot of local slot 0 (slot window of the block; 0 without a time window)
 };
@@ -1217,7 +1216,7 @@ struct AggSlow {  // what the out-of-line paths need (lives in local memory)
 __device__ __noinline__ void hist_bucket_general(const AggSlow* A, uint32_t g, long long v) {
   for (int s = 0; s < A->nsub; s++) {
     const KSubHist S = A->sub[s];
-    if (A->nsub > 1) {
+    if (A->multi) {  // a value in (Max, 10*Max] passes the MultiHist's reject rule but lies in no sub-range
       if (v < S.lo || v > S.hi) continue;
       if (v > S.reject_hi || v < S.lo) break;  // the subhist's own reject rule
     }
@@ -1238,13 +1237,11 @@ __device__ __noinline__ void agg_slow(const AggSlow* A, uint32_t g, long long v,
     return;
   }
   if (A->acc_smem) {
-    const uint32_t w = A->acc_w0_s + g * A->gstride_b;
-    if (count_accepted) sred_add(w, 1u);
-    const uint32_t lo = (uint32_t)(unsigned long long)v;
-    uint32_t hi = (uint32_t)((unsigned long long)v >> 32);
-    const uint32_t old = satom_add(w + A->R_b, lo);
-    if (old > ~lo) hi += 1u;  // carry out of the low limb
-    if (hi) sred_add(A->hi_s + g * A->hi_stride_b, hi);
+    if (count_accepted) sred_add(A->acc_w0_s + g * A->gstride_b, 1u);
+    // the value goes straight to the CTA's 64-bit total of the slot (shared memory; the fold between blocks
+    // runs between barriers): in the replicated low limb its low word (up to 2^32-1 for a negative value)
+    // would void the `nocarry` bound, and a later hot-path add would drop its carry
+    atomicAdd(A->csum + (size_t)(g + A->tb) * A->ctw, (unsigned long long)v);
   } else {
     gred_add(A->hcount + g + A->tb, 1ull);
     gred_add(A->sum + g + A->tb, (unsigned long long)v);
@@ -2026,6 +2023,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
       AS.info_max = KA->info_max;
       AS.reject_hi = KA->reject_hi;
       AS.nsub = KA->nsub;
+      AS.multi = (int)KA->multi;
       AS.nvals_total = KA->nvals_total;
       AS.buckets = reinterpret_cast<unsigned long long*>(KA->buckets);
       AS.hcount = reinterpret_cast<unsigned long long*>(KA->hcount);
@@ -2033,12 +2031,11 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
       AS.vmax = reinterpret_cast<long long*>(KA->vmax);
       AS.sub = KA->sub;
       AS.acc_w0_s = w0_s;
+      AS.csum = ctot + 2u + 2u * (uint32_t)ai;
+      AS.ctw = 1u + 2u * (uint32_t)naggs;
       const uint32_t hi_s = acc_s + (acc_rep + (uint32_t)ai) * 4u;  // + e * naggs * 4: this aggregation's high limb
       const uint32_t hi_stride_b = (uint32_t)naggs * 4u;
-      AS.hi_s = hi_s;
-      AS.hi_stride_b = hi_stride_b;
       AS.gstride_b = gstride_b;
-      AS.R_b = R_b;
       AS.acc_smem = ACC_SMEM ? 1 : 0;
       AS.tb = tb;
       // fast range: values the hot path takes — accepted (>= info_min, <= info_max <= reject_hi),

@@ -1875,6 +1875,7 @@ int make_plan(sg_query* q, const std::vector<uint32_t>& list) {
     ka.info_max = a.info_max;
     ka.reject_hi = wmul10(a.info_max);
     ka.nsub = (int32_t)L.subs.size();
+    ka.multi = q->d.hist_kind == SG_HIST_MULTI ? 1u : 0u;
     ka.nvals_total = L.nvals_total;
     for (size_t s = 0; s < L.subs.size(); s++) ka.sub[s] = L.subs[s];
   }
@@ -2321,6 +2322,26 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list) {
     }
   }
   lp.tmaps = lp.stage_units ? t->d_tmaps : nullptr;
+  if (getenv("SG_PLAN_TRACE")) {  // SG_PLAN_TRACE=1: one line per launch on stderr, so a test can see which path it reached
+    const Plan& P = q->plan;
+    fprintf(stderr, "sg_plan: build=%s slot_bytes=%u acc_repl=%u fold_every=%u fail_mode=%u hist_rows=%u lslots=%u nslots=%u hashed=%d",
+            q->variant->name, q->slot_bytes, P.acc_repl, lp.fold_every, P.fail_mode, P.hist_rows, P.lslots, P.nslots,
+            q->hashed ? 1 : 0);
+    for (int a = 0; a < P.naggs; a++) {
+      // the same expressions as scan_kernel's fast range, `hist32` and `nocarry` (R = acc_repl there)
+      const KAgg& ka = P.aggs[a];
+      const long long fmin = ka.info_min > 0 ? ka.info_min : 0;
+      long long fmax = ka.info_max < 0xffffffffll ? ka.info_max : 0xffffffffll;
+      if (ka.reject_hi < fmax) fmax = ka.reject_hi;
+      const bool fast_any = P.acc_repl > 0 && fmax >= fmin;
+      const bool hist32 = ka.nsub == 1 && ka.sub[0].bsize > 0 && ka.sub[0].bsize < 0x100000000ll && ka.sub[0].lo == ka.info_min &&
+                          fast_any && (unsigned long long)fmax - (unsigned long long)ka.info_min < 0x100000000ull;
+      const bool nocarry = fast_any && (unsigned long long)fmax * (unsigned long long)(SG_BLOCK_ROWS / P.acc_repl) * lp.fold_every <
+                                           0x100000000ull;
+      fprintf(stderr, " agg%d=[fmin=%lld fmax=%lld hist32=%d nocarry=%d]", a, fmin, fmax, hist32 ? 1 : 0, nocarry ? 1 : 0);
+    }
+    fprintf(stderr, "\n");
+  }
   int grid = (int)std::min<size_t>((size_t)q->grid, std::max<size_t>(items.size(), 1));
   CUDA_TRY(c, cudaEventRecord(q->ev0, c->stream));
   int rc = q->variant->launch(lp, grid, c->stream);

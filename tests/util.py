@@ -159,7 +159,7 @@ def close(a, b, tol):
     return abs(a - b) <= tol * max(1.0, abs(a), abs(b))
 
 
-def compare_group(g, o, aggs, op_hist, where, loghist=False):
+def compare_group(g, o, aggs, op_hist, where, loghist=False, mean=True):
     assert g.GroupByKey == o.GroupByKey, where
     assert g.Count == o.Count, (where, "Count")
     assert g.Samples == o.Samples, (where, "Samples")
@@ -172,7 +172,9 @@ def compare_group(g, o, aggs, op_hist, where, loghist=False):
         assert gh is not None, (where, a, "missing hist")
         assert gh.TotalCount() == oh.Count, (where, a, "hist Count")
         assert gh.Sum() == oh.ExactSum, (where, a, "exact int64 sum")
-        assert close(gh.Mean(), oh.Avg, MEAN_TOL), (where, a, "mean", gh.Mean(), oh.Avg)
+        check_mean = mean(oh) if callable(mean) else mean
+        if check_mean:
+            assert close(gh.Mean(), oh.Avg, MEAN_TOL), (where, a, "mean", gh.Mean(), oh.Avg)
         if op_hist or loghist:
             assert gh.Min() == oh.Min, (where, a, "Min")
             assert gh.Max() == oh.Max, (where, a, "Max")
@@ -182,12 +184,15 @@ def compare_group(g, o, aggs, op_hist, where, loghist=False):
             # first-seen block result still held Outliers (Q9, oracle_ffi._group)
             assert gh.GetPercentiles() == oh.Percentiles, (where, a, "percentiles")
             assert gh.GetIntBuckets() == oh.IntBuckets, (where, a, "sparse buckets")
-            assert close(gh.StdDev(), oh.StdDev, STD_TOL), (where, a, "stddev", gh.StdDev(), oh.StdDev)
+            if check_mean:  # (the stddev is taken around the mean)
+                assert close(gh.StdDev(), oh.StdDev, STD_TOL), (where, a, "stddev", gh.StdDev(), oh.StdDev)
 
 
-def compare(qs, oq, q):
+def compare(qs, oq, q, mean=True):
     """GPU QuerySpec vs oracle result: keys, Count, Samples, hist Count, exact sums, Min/Max, bucket
-    counters and percentiles bit-exact; mean / stddev within the stated tolerance."""
+    counters and percentiles bit-exact; mean / stddev within the stated tolerance.  mean=False, or a predicate
+    on the oracle's histogram that is false, skips the mean and stddev of those histograms (DESIGN.md §7: the
+    mean diverges where the sum left int64, and the reference's turns NaN in some groups)."""
     op_hist = q.op == "hist"
     assert qs.MatchedCount == oq.MatchedCount, "MatchedCount"
     assert qs.BrokenBlocks == oq.BrokenBlocks, "broken blocks"
@@ -202,17 +207,17 @@ def compare(qs, oq, q):
         assert sorted(r.GroupByKey for r in qs.Sorted) == sorted(r.GroupByKey for r in want), "groups"
     assert set(qs.Results) == set(r.GroupByKey for r in want), "group keys"
     for k in qs.Results:
-        compare_group(qs.Results[k], oq.Results[k], q.aggs if not q.time_col else [], op_hist, ("Results", k), q.loghist)
+        compare_group(qs.Results[k], oq.Results[k], q.aggs if not q.time_col else [], op_hist, ("Results", k), q.loghist, mean)
     c, oc = qs.Cumulative, oq.Cumulative
     assert c.GroupByKey == oc.GroupByKey
     assert c.Count == oc.Count and c.Samples == oc.Samples, "Cumulative counts"
     if not q.time_col:
-        compare_group(c, oc, q.aggs, op_hist, ("Cumulative",), q.loghist)
+        compare_group(c, oc, q.aggs, op_hist, ("Cumulative",), q.loghist, mean)
     assert set(qs.TimeResults) == set(oq.TimeResults), "time buckets"
     for tb, m in oq.TimeResults.items():
         assert set(qs.TimeResults[tb]) == set(m), ("time groups", tb)
         for k, o in m.items():
-            compare_group(qs.TimeResults[tb][k], o, q.aggs, op_hist, ("TimeResults", tb, k), q.loghist)
+            compare_group(qs.TimeResults[tb][k], o, q.aggs, op_hist, ("TimeResults", tb, k), q.loghist, mean)
 
 
 def random_spec(seed, nrows=3000, block_rows=1000, nulls=True, threshold=5000, wide=False, sets=False):
