@@ -344,8 +344,8 @@ def query(blocks, key_types, filters, groups, aggs, op_hist=False, log_hist=Fals
                     if key_types[slot] == F.SG_COL_STR:
                         tab = cols[slot][1].string_table
                         key.append((tab[v] if 0 <= v < len(tab) else b"").decode())
-                    else:
-                        key.append(str(v))
+                    else:  # uint64(-1) is MISSING_VALUE: -1 renders as missing (aggregate.go:125-143,306)
+                        key.append("" if v == -1 else str(v))
                 else:
                     key.append("")
             skey = "".join(k + "\t" for k in key) if groups else "total"

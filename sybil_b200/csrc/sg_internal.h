@@ -89,7 +89,10 @@ struct KGroup {
   const long long* vh_keys;
   const uint32_t* vh_ids;
   uint32_t vh_mask;  // capacity - 1
-  uint32_t _pad;
+  // the global id (str) / value-dictionary code (int) whose key renders like a missing value and so takes code 0
+  // with the missing rows: the int -1 (uint64(-1) is MISSING_VALUE, aggregate.go:125-143) and the string "";
+  // -1 when the dictionary holds neither
+  int32_t alias;
 };
 
 struct KSubHist {  // one BasicHist bucket layout (hist_basic.go:34-70)

@@ -1064,8 +1064,8 @@ __device__ __forceinline__ void slot_or(SlotT* slot, uint32_t slot_s, uint32_t r
     asm volatile("red.shared.or.b32 [%0], %1;" ::"r"(slot_s + (row & ~3u)), "r"(v << ((row & 3u) << 3)) : "memory");
   else if (sizeof(SlotT) == 2)
     asm volatile("red.shared.or.b32 [%0], %1;" ::"r"(slot_s + ((row & ~1u) << 1)), "r"(v << ((row & 1u) << 4)) : "memory");
-  else
-    slot[row] = (SlotT)(slot[row] | v);
+  else  // atomic too: a set column lists a row in as many bins as its set has tags, walked by different threads
+    atomicOr(reinterpret_cast<unsigned int*>(slot) + row, v);
 }
 
 // value-array str column (raw int32 local ids): visit(row, local_id)
@@ -1772,7 +1772,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
         count_in_group = ACC_SMEM && nfilters == 0 && time_col < 0 && ngroups == 1 && (c.flags & COL_FULL) != 0u;
         for (uint32_t b = cx.tid; b < c.nbins; b += THREADS) {
           const int32_t code = G.is_str ? str_gid(c, c.bin_values[b]) : c.remap[b];
-          pay[b] = ((uint32_t)code + 1u) * G.stride;
+          pay[b] = code == G.alias ? 0u : ((uint32_t)code + 1u) * G.stride;
           if (count_in_group)
             sred_add(smem_u32(cx.acc + pay[b] * gstride + lane_off), c.bin_offsets[b + 1] - c.bin_offsets[b]);
         }
@@ -1790,16 +1790,17 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
         }
       } else if (c.enc == SG_ENC_VALUES && G.is_str) {
         const uint32_t stride = G.stride;
+        const int32_t alias = G.alias;
+        auto word = [&](int32_t local) {
+          const int32_t gid = str_gid(c, local);
+          return gid == alias ? 0u : ((uint32_t)gid + 1u) * stride;
+        };
         if (nfilters == 0 && gi == 0) {
           // first pass to touch the zeroed slot words: a store, not a read-modify-write (with the slot words in
           // the global scratch the load was the top stall of the high-cardinality plan)
-          scan_values_i32(cx, c, nrec, [&](uint32_t row, int32_t local) {
-            slot[row] = (SlotT)(((uint32_t)str_gid(c, local) + 1u) * stride);
-          });
+          scan_values_i32(cx, c, nrec, [&](uint32_t row, int32_t local) { slot[row] = (SlotT)word(local); });
         } else {
-          scan_values_i32(cx, c, nrec, [&](uint32_t row, int32_t local) {
-            slot[row] = (SlotT)(slot[row] + ((uint32_t)str_gid(c, local) + 1u) * stride);
-          });
+          scan_values_i32(cx, c, nrec, [&](uint32_t row, int32_t local) { slot[row] = (SlotT)(slot[row] + word(local)); });
         }
       }
       else if (HASHG && c.enc == SG_ENC_VALUES && !G.is_str) {
@@ -1826,7 +1827,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
                 cx.misc[1] = 1;
                 id = 0u;
               }
-              inc[k] = (id + 1u) * stride;
+              inc[k] = id == (uint32_t)G.alias ? 0u : (id + 1u) * stride;
             }
           }
           add_slots(slot, idx0, inc);
@@ -2132,12 +2133,12 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
           if (nvalid < VE) {
 #pragma unroll
             for (int k = 0; k < VE; k++)
-              if (k >= nvalid) sw[k] = NOFILT ? trash : ~0u;  // rows past len(Values): handled by the tail loop below
+              if (k >= nvalid) sw[k] = NOFILT ? trash : ~passbits;  // rows past len(Values): handled by the tail loop below
           }
           if (DO_COUNT && count_matched) {
 #pragma unroll
             for (int k = 0; k < VE; k++)
-              if (((sw[k] >> gbits) & filt_mask) == filt_target && sw[k] != ~0u) my_matched++;
+              if (k < (int)nvalid && ((sw[k] >> gbits) & filt_mask) == filt_target) my_matched++;
           }
           uint32_t cmask = 0, slow_any = 0;
 #pragma unroll
@@ -2287,12 +2288,14 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
           if (nvalid < VE) {
 #pragma unroll
             for (int k = 0; k < VE; k++)
-              if (k >= nvalid) sw[k] = ~0u;  // rows past len(Values): handled by the tail loop below
+              // rows past len(Values), handled by the tail loop below, take a word that maps to trash and fails the
+              // filters (~0 would not: it is the highest slot's passing word when the slot word fills 32 bits)
+              if (k >= nvalid) sw[k] = ~passbits;
           }
           if (DO_COUNT && count_matched) {
 #pragma unroll
             for (int k = 0; k < VE; k++)
-              if (((sw[k] >> gbits) & filt_mask) == filt_target && sw[k] != ~0u) my_matched++;
+              if (k < (int)nvalid && ((sw[k] >> gbits) & filt_mask) == filt_target) my_matched++;
           }
           if (ACC_SMEM && fast_any) {
             uint32_t cmask = 0, slow_any = 0;

@@ -1649,6 +1649,17 @@ int make_plan(sg_query* q, const std::vector<uint32_t>& list) {
     P.groups[i].is_str = gd.is_str;
     P.groups[i].stride = gd.stride;
     P.groups[i].radix = gd.radix;
+    // a key that renders like a missing value is the missing group (DESIGN.md §7): the int -1 and the string ""
+    // take code 0.  Not on the weight axis (a weight of -1 multiplies), nor on a StrReplace column (its rewritten
+    // strings are folded on the host)
+    P.groups[i].alias = -1;
+    if (gd.is_str && !gd.is_weight && !q->repl.count(gd.col)) {
+      P.groups[i].alias = t->sdict[(size_t)gd.col].find(std::string());
+    } else if (!gd.is_str && !gd.is_weight) {
+      const auto& m = t->idict[(size_t)gd.col].map;
+      const auto it = m.find(-1);
+      if (it != m.end()) P.groups[i].alias = it->second;
+    }
   }
   if (time_mode) {
     if (!col_ok(P.time_col) || t->types[(size_t)P.time_col] != SG_COL_INT) {
@@ -1688,7 +1699,9 @@ int make_plan(sg_query* q, const std::vector<uint32_t>& list) {
   // ---- hashed slot space: more codes than dense slots.  The table gets twice as many entries as rows can make
   // groups (every scanned row its own group at worst), within [2^16, 2^26]; a table that fills up fails the query.
   q->code_space = stride;
-  q->hashed = stride > (uint64_t)MAX_SLOTS && !getenv("SG_NO_HASHED_SLOTS");
+  // tests: SG_FORCE_HASHED_SLOTS=1 takes the hashed slot space at any size (it must give what the dense one gives);
+  // SG_HASH_CAP_LOG2=n caps its table at 2^n entries, so that a table that fills up can be reached with few rows
+  q->hashed = (stride > (uint64_t)MAX_SLOTS || getenv("SG_FORCE_HASHED_SLOTS")) && !getenv("SG_NO_HASHED_SLOTS");
   if (stride > (uint64_t)MAX_SLOTS && !q->hashed) {
     c->set_err("query: group-by cardinality product exceeds the dense slot space");
     return SG_ERR_UNSUPPORTED;
@@ -1696,8 +1709,10 @@ int make_plan(sg_query* q, const std::vector<uint32_t>& list) {
   if (q->hashed) {
     uint64_t rows = 0;
     for (uint32_t b : list) rows += t->blocks[b].num_records;
-    uint64_t cap = (uint64_t)1 << 16;
-    while (cap < 2 * std::min<uint64_t>(rows, stride) && cap < (uint64_t)MAX_SLOTS) cap <<= 1;
+    uint64_t cap_max = (uint64_t)MAX_SLOTS;
+    if (const char* e = getenv("SG_HASH_CAP_LOG2")) cap_max = (uint64_t)1 << std::min(std::max(atoi(e), 4), 26);
+    uint64_t cap = std::min<uint64_t>((uint64_t)1 << 16, cap_max);
+    while (cap < 2 * std::min<uint64_t>(rows, stride) && cap < cap_max) cap <<= 1;
     P.nslots = (uint32_t)cap;
   }
   // ---- fail mode: every filter column populates every row of every listed block (value array, or a
@@ -1755,9 +1770,9 @@ int make_plan(sg_query* q, const std::vector<uint32_t>& list) {
     P.gbits = bits_for(P.lslots);
   };
   window_for(!q->hashed);
-  if (q->hashed) {  // the slot word carries the whole code; the accumulators are indexed by the table index
+  if (q->hashed) {  // the slot word carries the whole code, then the table index the accumulators are indexed by
     P.lslots = P.nslots;
-    P.gbits = bits_for(q->code_space);
+    P.gbits = bits_for(std::max<uint64_t>(q->code_space, P.nslots));  // (the table outgrows a forced small space)
   }
   P.time_magic = 0;
   if (time_mode && P.time_bucket >= 2 && P.time_bucket < 0x100000000ll)
@@ -2324,9 +2339,18 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list) {
   lp.tmaps = lp.stage_units ? t->d_tmaps : nullptr;
   if (getenv("SG_PLAN_TRACE")) {  // SG_PLAN_TRACE=1: one line per launch on stderr, so a test can see which path it reached
     const Plan& P = q->plan;
-    fprintf(stderr, "sg_plan: build=%s slot_bytes=%u acc_repl=%u fold_every=%u fail_mode=%u hist_rows=%u lslots=%u nslots=%u hashed=%d",
+    // (the slot word: gbits group bits, fbits pass-counter / fail and set-filter bits, tbit time bit)
+    // count_bins: listed blocks whose group Count the kernel takes from bin sizes (its count_in_group conditions)
+    uint32_t count_bins = 0;
+    if (P.acc_repl > 0 && P.nfilters == 0 && P.time_col < 0 && P.ngroups == 1)
+      for (uint32_t b : list) {
+        const DevCol& dc = t->cols[(size_t)b * (size_t)t->ncols + (size_t)P.groups[0].col];
+        count_bins += dc.enc == SG_ENC_BUCKET && (dc.flags & COL_FULL) ? 1u : 0u;
+      }
+    fprintf(stderr, "sg_plan: build=%s slot_bytes=%u acc_repl=%u fold_every=%u fail_mode=%u hist_rows=%u lslots=%u nslots=%u hashed=%d"
+            " hashg=%d gbits=%u fbits=%d tbit=%d count_bins=%u",
             q->variant->name, q->slot_bytes, P.acc_repl, lp.fold_every, P.fail_mode, P.hist_rows, P.lslots, P.nslots,
-            q->hashed ? 1 : 0);
+            q->hashed ? 1 : 0, q->hashg ? 1 : 0, P.gbits, __builtin_popcount(P.filt_mask), P.time_ok ? 1 : 0, count_bins);
     for (int a = 0; a < P.naggs; a++) {
       // the same expressions as scan_kernel's fast range, `hist32` and `nocarry` (R = acc_repl there)
       const KAgg& ka = P.aggs[a];
@@ -2751,7 +2775,8 @@ static int build_result_topk(sg_query* q, sg_result** out) {
 // StrReplace: strings of a group column that rewrite to the same text are one group in the reference (the block's
 // string table is rewritten before any row is read, column_store_io.go:529-547).  The scan grouped by the original
 // global ids; every dense slot whose code on a rewritten axis is not its class representative is added onto the
-// representative's slot (counts, hist counts, sums, bucket counters: +; max: max) and cleared.
+// representative's slot (counts, hist counts, sums, bucket counters: +; max: max) and cleared.  A string that
+// rewrites to "" goes onto code 0 instead: it renders like a missing value, and is the missing group (DESIGN.md §7).
 //
 // Weights (OPTS.WEIGHT_COL): the scan grouped by the weight value as a hidden last axis (make_plan); the slots of
 // weight w are multiplied by w and added onto code 0 of that axis — Count / hist Count / Values[] += weight
@@ -2764,6 +2789,7 @@ static int fold_axes(sg_query* q, uint64_t* h, size_t have, sg_result* r, int64_
     const GroupDim& d = q->dims[di];
     if (d.is_time) continue;
     const std::vector<uint32_t>* canon = nullptr;
+    const std::vector<std::string>* rtext = nullptr;  // StrReplace: the rewritten text of every global id
     std::vector<uint64_t> wmul;  // weight axis: multiplier per code - 1
     if (d.is_weight) {
       const std::vector<int64_t>& vals = q->merged ? q->m_ints[di] : q->table->idict[(size_t)d.col].vals;
@@ -2791,7 +2817,8 @@ static int fold_axes(sg_query* q, uint64_t* h, size_t have, sg_result* r, int64_
       auto it = q->repl.find(d.col);
       if (it == q->repl.end()) continue;
       canon = &it->second.canon;
-      if (canon->size() + 1 != (size_t)d.radix) {
+      rtext = &it->second.strs;
+      if (canon->size() + 1 != (size_t)d.radix || rtext->size() != canon->size()) {
         c->set_err("query: the dictionary of a StrReplace column grew after sg_query_set_str_replace");
         return SG_ERR_STATE;
       }
@@ -2805,7 +2832,9 @@ static int fold_axes(sg_query* q, uint64_t* h, size_t have, sg_result* r, int64_
         if (code == 0) continue;
         uint32_t to;
         uint64_t mul = 1;
-        if (canon) {
+        if (canon && (*rtext)[code - 1].empty()) {
+          to = s - code * d.stride;  // rewritten to "": the missing group, which renders alike (DESIGN.md §7)
+        } else if (canon) {
           if ((*canon)[code - 1] == code - 1) continue;
           to = s - (code - 1 - (*canon)[code - 1]) * d.stride;
         } else {

@@ -472,11 +472,13 @@ class Table:
         qs.Cumulative = allg[0]
         qs.Sorted = allg[1:]
         qs.Results = {r.GroupByKey: r for r in qs.Sorted}
-        qs.TimeResults = {}
+        qs.TimeResults, qs.TimeNumGroups = {}, {}
         for b in range(lib.sg_result_num_time_buckets(rp)):
             tb = lib.sg_result_time_bucket(rp, b)
             sl = _ResultHandle(lib, lib.sg_result_time_slice(rp, b))
-            qs.TimeResults[tb] = {r.GroupByKey: r for r in sl.groups(qs.Aggregations, False)}
+            groups = sl.groups(qs.Aggregations, False)
+            qs.TimeResults[tb] = {r.GroupByKey: r for r in groups}
+            qs.TimeNumGroups[tb] = len(groups)  # (a key two groups shared would count once in the dict)
 
 
 class PreparedQuery:

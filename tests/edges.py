@@ -9,20 +9,22 @@ shows it reached the path it targets."""
 import numpy as np
 
 from tests.rowref import I64_MAX, I64_MIN, basic_layout, i64
-from tests.util import INT, STR, Q, Spec
+from tests.util import INT, SET, STR, Q, Spec
 
 KT = [("g", STR), ("k", INT), ("w", INT), ("t", INT)] + [("v%d" % i, INT) for i in range(9)]
 
 
 class _Table:
-    def __init__(self, forms=None):
-        self.spec = Spec(KT)
+    def __init__(self, forms=None, kt=KT):
+        self.spec = Spec(kt)
         self.spec.forms = forms
         self.rows, self.valid = [], []
 
     def add(self, cols, valid=None, block_rows=None, threshold=5000):
-        cols = {k: (np.asarray(v, np.int64) if self.spec.KeyTypes[self.spec.KeyTable[k]] == INT else np.asarray(v))
-                for k, v in cols.items()}
+        def arr(k, v):
+            typ = self.spec.KeyTypes[self.spec.KeyTable[k]]
+            return np.asarray(v, np.int64) if typ == INT else (list(v) if typ == SET else np.asarray(v))
+        cols = {k: arr(k, v) for k, v in cols.items()}
         self.spec.add_rows(cols, valid, threshold=threshold, block_rows=block_rows)
         self.rows.append((cols, block_rows, threshold))
         self.valid.append(valid or {})
@@ -322,6 +324,330 @@ def family_f(forms=None):
     return t.done(qs)
 
 
+# ---------------------------------------------------------------------------------------------------------------
+# G. Key identity and rendering
+# ---------------------------------------------------------------------------------------------------------------
+# The key side of the scan: a row's group key becomes a dictionary code, the codes a mixed-radix slot, the slot a
+# rendered GroupByKey.  An int -1 is uint64(-1) = MISSING_VALUE in the reference (aggregate.go:125-143), so it is
+# the missing group; INT64_MIN is the device value set's empty marker; values above 2^32 do not fit a 32-bit code.
+G_KEYS = [-1, 0, I64_MIN, I64_MAX, (1 << 32) + 7, (1 << 40) + 1, -2]
+# rows per key in each bucket-encoded block (None: rows without the column).  Missing and -1 are one group of 250
+# rows, the largest; apart they would sort fifth (-1) and sixth (missing)
+G_COUNTS = {None: 120, -1: 130, 0: 240, I64_MIN: 230, I64_MAX: 220, (1 << 32) + 7: 210, (1 << 40) + 1: 60, -2: 50}
+KT_KEYS = ([("g", STR), ("s", STR), ("s2", STR), ("k", INT), ("t", INT), ("v0", INT), ("f", INT), ("f2", INT), ("tags", SET)] +
+           [(c, INT) for c in "abcdeqrp"])
+
+
+def _g_block(rng):
+    keys = [k for k, c in G_COUNTS.items() for _ in range(c)]
+    keys = [keys[i] for i in rng.permutation(len(keys))]
+    k = np.array([0 if x is None else x for x in keys], np.int64)
+    return k, np.array([x is not None for x in keys])
+
+
+def _g_queries(s, expect, radix=()):
+    # radix: (lslots of ["k"], of ["g", "k"]) when the dictionaries are known: k's 7 keys + missing, g's 2 strings +
+    # the "" staging interns + missing
+    e0, e1 = ([r"lslots=%d " % radix[0]], [r"lslots=%d " % radix[1]]) if radix else ([], [])
+    return [
+        _q(s, groups=["k"], aggs=["v0"], op="avg", expect=expect + e0),
+        _q(s, groups=["g", "k"], aggs=["v0"], op="hist", expect=expect + e1),
+        _q(s, groups=["k", "g"], aggs=["v0"], op="avg", expect=expect),
+        _q(s, groups=["k"], aggs=["v0"], op="avg", time_col="t", time_bucket=500, expect=expect),
+        _q(s, groups=["g", "k"], aggs=[], op="avg", time_col="t", time_bucket=1 << 20, expect=expect),
+        # the merge of -1 into the missing group must come before the top-K: merged it is the first group
+        _q(s, groups=["k"], aggs=["v0"], op="avg", limit=3, expect=expect),
+        _q(s, int_filters=[("v0", "gt", 10)], groups=["k"], aggs=["v0"], op="avg", limit=2, expect=expect),
+    ]
+
+
+def family_g_int(mixed, forms=None):
+    """The int keys of G_KEYS next to missing rows.  Bucket-encoded only (dictionary codes from the bins), or
+    mixed with value-array blocks (the device value dictionary: distinct_kernel + vh_keys) that hold the same keys,
+    a spread of filler keys, gaps that read 0 and are populated, and rows past len(Values)."""
+    rng = np.random.default_rng(20 + mixed)
+    t = _Table(forms, KT_KEYS)
+    for _ in range(2):
+        k, valid = _g_block(rng)
+        n = len(k)
+        t.add({"g": _groups(rng, n, 2), "k": k, "t": rng.integers(0, 1500, n), "v0": rng.integers(0, 100, n)},
+              {"k": valid})
+    if mixed:
+        n = 3000
+        k = np.where(rng.random(n) < 0.5, rng.choice(np.asarray(G_KEYS, np.int64), n), 1000 + np.arange(n))
+        valid = rng.random(n) > 0.05  # the gaps read 0
+        valid[-100:] = False  # past len(Values): missing
+        k[0] = -1
+        t.add({"g": _groups(rng, n, 2), "k": k, "t": rng.integers(0, 1500, n), "v0": rng.integers(0, 100, n)},
+              {"k": valid}, threshold=50, block_rows=1500)
+    t.extents(v0=(0, 100))
+    return t.done(_g_queries(t.spec, [r"hashg=1"] if mixed else [r"hashg=0 .*gbits=\d"], () if mixed else (8, 32)))
+
+
+def family_g_str(forms=None):
+    """A str column holding "" next to rows without it, bucket-encoded and as value arrays (whose gaps read the
+    block's first string, here "").  The reference renders both as "" and then keeps one of the two groups per
+    block, whichever its map iteration visits last (translate_group_by, aggregate.go:284-324), so its answer is
+    not deterministic; the engine merges them, as tests/rowref.py and pyoracle do.  These queries carry
+    oracle=False: the C++ oracle, which keeps one of the two like the reference, is not compared."""
+    rng = np.random.default_rng(23)
+    t = _Table(forms, KT_KEYS)
+    n = 1200
+    for thr in (5000, 40):
+        s = rng.choice(np.asarray(["", "a", "b"]), n)
+        if thr < 5000:
+            s = np.where(rng.random(n) < 0.5, s, np.asarray(["x%d" % i for i in range(n)]))
+            s[0] = ""
+        valid = rng.random(n) > 0.1
+        valid[0] = True
+        t.add({"g": _groups(rng, n, 2), "s": s, "t": rng.integers(0, 1500, n), "v0": rng.integers(0, 100, n)},
+              {"s": valid}, threshold=thr)
+    t.extents(v0=(0, 100))
+    s = t.spec
+    dense = [r"hashed=0 hashg=0 "]
+    qs = [_q(s, groups=["s"], aggs=["v0"], op="avg", expect=dense),
+          _q(s, groups=["g", "s"], aggs=["v0"], op="hist", expect=dense),
+          _q(s, groups=["s"], aggs=["v0"], op="avg", time_col="t", time_bucket=500, expect=dense + [r"tbit=1"]),
+          _q(s, groups=["s"], aggs=["v0"], op="avg", limit=2, expect=dense)]
+    for q in qs:
+        q.oracle = False
+    return t.done(qs)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# H. Slot-word widths
+# ---------------------------------------------------------------------------------------------------------------
+# int group columns of a given number of distinct values (radix = that + 1, code 0 missing): radices 16, 16, 17,
+# 256, 256, 8, 8, 2.  Every block holds every value, and one row sits on every axis' highest code at once
+H_DISTINCT = {"a": 15, "b": 15, "c": 16, "d": 255, "e": 255, "q": 7, "r": 7, "p": 1}
+H_TAGS = ["t%d" % i for i in range(14)]
+
+
+def _h_word(gbits, fbits, tbit, nbytes):
+    return r"slot_bytes=%d .*gbits=%d fbits=%d tbit=%d" % (nbytes, gbits, fbits, tbit)
+
+
+def family_h(forms=None):
+    """Group axes whose radix products put gbits + fbits + tbit on 8 / 9, 16 / 17 and 32 bits: no filter, fail mode
+    (f is in every row), count mode with 1, 3 and 4 counting filters (f2 misses rows), IN / NIN sticky bits, with and
+    without the time bit (every block inside one time bucket: a window of one code, so lslots = 2 x the group slots).
+    The widest query passes the slot word 0xFFFFFFFF for legitimate rows in blocks whose v0 array ends early."""
+    rng = np.random.default_rng(24)
+    t = _Table(forms, KT_KEYS)
+    n = 4096
+    for blk in range(3):
+        cols, valid = {}, {}
+        for c, m in H_DISTINCT.items():
+            v = rng.integers(0, m, n)
+            v[:m] = np.arange(m)  # every value in every block
+            v[300:364] = m - 1  # rows on the highest code of every axis
+            cols[c] = v
+            va = rng.random(n) > 0.02
+            va[:364] = True
+            va[-3:] = False  # rows on code 0 of every axis
+            valid[c] = va
+        cols["f"] = rng.integers(0, 10, n)
+        cols["f2"] = rng.integers(0, 10, n)
+        valid["f2"] = rng.random(n) > 0.1
+        valid["f2"][:1024] = True
+        tags = [list(H_TAGS) if i < 512 or rng.random() < 0.3 else list(rng.choice(H_TAGS, 3, replace=False))
+                for i in range(n)]
+        cols["tags"] = tags
+        valid["tags"] = rng.random(n) > 0.05
+        valid["tags"][:1024] = True
+        cols["t"] = np.full(n, 1000 * blk + 10)
+        # v0 a value array (threshold 300 < its distinct values) whose len(Values) ends 40 rows before the block
+        cols["v0"] = rng.integers(0, 1000, n)
+        valid["v0"] = np.ones(n, bool)
+        valid["v0"][-40:] = False
+        t.add(cols, valid, threshold=300)
+    t.extents(v0=(0, 1000))
+    s = t.spec
+    ins = [("tags", "in", x) for x in H_TAGS]
+    f1, f2 = [("f", "gt", -1)], [("f2", "gt", -1)]
+    f3 = f2 + [("f2", "lt", 9), ("f2", "neq", 5)]
+    f4 = f3 + [("f2", "neq", 7)]
+    tm = dict(time_col="t", time_bucket=1000)
+    avg = dict(aggs=["v0"], op="avg")
+    qs = [
+        _q(s, groups=["a", "b"], expect=[_h_word(8, 0, 0, 1)], **avg),
+        _q(s, groups=["a", "c"], expect=[_h_word(9, 0, 0, 2)], **avg),
+        _q(s, groups=["d", "e"], expect=[_h_word(16, 0, 0, 2)], **avg),
+        _q(s, groups=["d", "e", "p"], expect=[_h_word(17, 0, 0, 4)], **avg),
+        _q(s, int_filters=f1, groups=["a", "q"], expect=[_h_word(7, 1, 0, 1), "fail_mode=1"], **avg),
+        _q(s, int_filters=f1, groups=["a", "b"], expect=[_h_word(8, 1, 0, 2), "fail_mode=1"], **avg),
+        _q(s, int_filters=f1, groups=["d", "a"], expect=[_h_word(12, 1, 0, 2), "fail_mode=1"], **avg),
+        _q(s, int_filters=f2, groups=["a", "q"], expect=[_h_word(7, 1, 0, 1), "fail_mode=0"], **avg),
+        _q(s, int_filters=f2, groups=["a", "b"], expect=[_h_word(8, 1, 0, 2), "fail_mode=0"], **avg),
+        _q(s, int_filters=f3, groups=["q", "r"], expect=[_h_word(6, 2, 0, 1)], **avg),
+        _q(s, int_filters=f3, groups=["a", "q"], expect=[_h_word(7, 2, 0, 2)], **avg),
+        _q(s, int_filters=f4, groups=["d", "a", "p"], expect=[_h_word(13, 3, 0, 2)], **avg),
+        _q(s, int_filters=f4, groups=["d", "c", "p"], expect=[_h_word(14, 3, 0, 4)], **avg),
+        _q(s, set_filters=ins[:1], groups=["a", "q"], expect=[_h_word(7, 1, 0, 1)], **avg),
+        _q(s, set_filters=[("tags", "nin", "zz")], groups=["a", "q"], expect=[_h_word(7, 2, 0, 2)], **avg),
+        _q(s, set_filters=[("tags", "nin", "t3")], groups=["q", "r"], expect=[_h_word(6, 2, 0, 1)], **avg),
+        _q(s, groups=["q", "r"], expect=[_h_word(7, 0, 1, 1)], **avg, **tm),
+        _q(s, groups=["a", "q"], expect=[_h_word(8, 0, 1, 2)], **avg, **tm),
+        _q(s, int_filters=f1, groups=["a", "r"], expect=[_h_word(8, 1, 1, 2)], **avg, **tm),
+        # 17 group bits + 1 pass-counter bit + 14 IN bits: the highest slot's passing rows have the word 0xFFFFFFFF
+        _q(s, int_filters=f2, set_filters=ins, groups=["d", "e", "p"], expect=[_h_word(17, 15, 0, 4)], **avg),
+        _q(s, int_filters=f2, set_filters=ins, groups=["d", "e", "p"], op="hist", aggs=["v0"],
+           expect=[_h_word(17, 15, 0, 4)]),
+    ]
+    return t.done(qs)
+
+
+def h_refused(spec):
+    """The widest H layout plus the time bit: 33 bits, refused ("slot word wider than 32 bits")."""
+    return _q(spec, int_filters=[("f2", "gt", -1)], set_filters=[("tags", "in", x) for x in H_TAGS],
+              groups=["d", "e", "p"], aggs=["v0"], op="avg", time_col="t", time_bucket=1000)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# K. Thresholds inside the pass
+# ---------------------------------------------------------------------------------------------------------------
+K_BINS = [1023, 1024, 1025]  # per-bin payload: in shared memory up to SMEM_BINS = 1024 bins, then in gbinpay
+
+
+def family_k(forms=None):
+    """A bucket-encoded group column and filter column with 1,023 / 1,024 / 1,025 bins in one block each, and a
+    group column in every row of its blocks (count from bin sizes, COL_FULL) next to the same with one row missing."""
+    rng = np.random.default_rng(25)
+    t = _Table(forms, KT_KEYS)
+    for nb in K_BINS:
+        n = 8192
+        k = rng.integers(0, nb, n)
+        k[:nb] = np.arange(nb)
+        f = rng.integers(0, nb, n)
+        f[:nb] = np.arange(nb)
+        t.add({"g": _groups(rng, n, 2), "k": k * 7 - 3000, "f": f, "v0": rng.integers(0, 100, n)},
+              threshold=nb)
+    for miss in (False, True):
+        n = 5000
+        a = rng.integers(0, 40, n)
+        va = np.ones(n, bool)
+        va[1234] = not miss
+        t.add({"g": _groups(rng, n, 3), "a": a, "v0": rng.integers(0, 100, n)}, {"a": va})
+    t.extents(v0=(0, 100))
+    s = t.spec
+    return t.done([
+        # count_bins: the blocks whose Count comes from bin sizes (the three k blocks list every row once)
+        _q(s, groups=["k"], aggs=["v0"], op="avg", expect=[r"count_bins=3\b"]),
+        _q(s, int_filters=[("f", "gt", 100)], groups=["k"], aggs=["v0"], op="avg", expect=[r"count_bins=0\b"]),
+        _q(s, int_filters=[("f", "lt", 1000)], groups=["g", "k"], aggs=["v0"], op="hist", expect=[r"count_bins=0\b"]),
+        # the a block without a missing row takes the shortcut, the one with a missing row does not
+        _q(s, groups=["a"], aggs=["v0"], op="avg", expect=[r"count_bins=1\b"]),
+        _q(s, groups=["a"], aggs=[], op="avg", expect=[r"count_bins=1\b"]),
+    ])
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# I. The dense / hashed switch and the code ceiling
+# ---------------------------------------------------------------------------------------------------------------
+def slot_hash(x):
+    """sybil_b200/csrc/sg_internal.h slot_hash, restated over uint32 numpy arrays: the hashed slot space probes
+    from slot_hash(code + 1) & hmask.  The collision chains of family_i_ceiling depend on this function."""
+    x = np.asarray(x, np.uint32)
+    with np.errstate(over="ignore"):
+        x = x ^ (x >> np.uint32(16))
+        x = x * np.uint32(0x7feb352d)
+        x = x ^ (x >> np.uint32(15))
+        x = x * np.uint32(0x846ca68b)
+        x = x ^ (x >> np.uint32(16))
+    return x
+
+
+def _strs(prefix, n):
+    return np.array(["%s%05d" % (prefix, i) for i in range(n)])
+
+
+def family_i_dense(plus, forms=None):
+    """Two str axes of radix 8192 each: 8,189 strings in a first block (then the "" staging interns) and one more
+    in a second block, whose row sits on the last slot of the 2^26 dense slots.  plus: a third block adds one more s
+    string, radix 8192 x 8193 = 2^26 + 8192 codes: hashed, its table at the 2^16 minimum.  (2^26 + 1 = 5 x
+    13,421,773 would need 13M strings on one axis; 8192 x 8193 is the smallest product of these axes past 2^26.)"""
+    rng = np.random.default_rng(26)
+    t = _Table(forms, KT_KEYS)
+    n = 8189
+    g, s = _strs("a", n + 2), _strs("b", n + 2)
+    t.add({"g": g[:n], "s": rng.permutation(s[:n]), "v0": rng.integers(0, 100, n)})
+    # the last slot on 3 rows, the largest group (a tie-free top-1)
+    t.add({"g": np.array([g[n], g[n], g[n], g[0]]), "s": np.array([s[n]] * 4), "v0": [7, 8, 9, 10]})
+    if plus:
+        t.add({"g": np.array([g[n]]), "s": np.array([s[n + 1]]), "v0": [9]})
+    t.extents(v0=(0, 100))
+    sp = t.spec
+    expect = ([r"lslots=65536 nslots=65536 hashed=1 hashg=0 gbits=27 fbits=0 tbit=0 "] if plus else
+              [r"lslots=67108864 nslots=67108864 hashed=0 hashg=0 gbits=26 fbits=0 tbit=0 "])
+    return t.done([_q(sp, groups=["g", "s"], aggs=[], op="avg", expect=expect),
+                   _q(sp, groups=["s", "g"], aggs=[], op="avg", limit=1, expect=expect)])
+
+
+def i_dense_hist(spec):
+    """A histogram over the 2^26 dense slots: 1,002 counters per slot, far past the 24 GiB accumulator limit."""
+    return _q(spec, groups=["g", "s"], aggs=["v0"], op="hist")
+
+
+I_CEIL = (42964, 49979)  # strings of g and s: radices 42,966 x 49,981 = 2^31 - 2 = MAX_CODE_SPACE
+
+
+def family_i_ceiling(forms=None):
+    """The 31-bit code ceiling.  A first block (f = 0) holds every string: g's 42,964, s's 49,979 and s2's 49,980
+    (radix 49,982: g x s2 is past 2^31 - 2).  Queries filter on f with eq, so zone maps drop that block and the
+    hashed table is sized by the rows of the blocks they list:
+    - f = 1: 160 rows on codes whose slot_hash lands on the last entries of the 2^16-entry table or on its first
+      ones, so probe chains wrap from hmask to 0 (each such key on 3 rows), plus random codes;
+    - f = 2 / 3: 32,768 / 32,769 random rows, 2 x rows just at / just past 2^16: tables of 2^16 / 2^17 entries.
+    With one filter in fail mode the slot word is 31 group bits + 1: exactly 32, accepted."""
+    rng = np.random.default_rng(31)
+    t = _Table(forms, KT_KEYS)
+    ng, ns = I_CEIL
+    n = ns + 1
+    g, s, s2 = _strs("a", ng), _strs("b", ns), _strs("c", n)
+    t.add({"g": np.resize(g, n), "s": np.resize(s, n), "s2": s2, "f": np.zeros(n, np.int64)})
+    # global ids follow first sight: g[i] -> i, s[i] -> i ("" comes after them); code = (ig + 1) + (is + 1) * 42966
+    ig = np.arange(ng, dtype=np.int64)
+    pick = []
+    for js in rng.choice(ns, 400, replace=False):
+        code = (ig + 1) + (int(js) + 1) * (ng + 2)
+        h = slot_hash((code + 1).astype(np.uint32)) & np.uint32(0xFFFF)
+        for want in (0xFFFF, 0xFFFE, 0xFFFD, 0, 1):
+            pick += [(int(i), int(js)) for i in np.nonzero(h == want)[0][:1]]
+    pick = pick[:40]
+    rows = [p for p in pick for _ in range(3)] + [(int(rng.integers(ng)), int(rng.integers(ns))) for _ in range(40)]
+    a, b = np.array([r[0] for r in rows]), np.array([r[1] for r in rows])
+    t.add({"g": g[a], "s": s[b], "f": np.ones(len(rows), np.int64), "v0": rng.integers(0, 100, len(rows))})
+    for f, m in ((2, 32768), (3, 32769)):
+        t.add({"g": g[rng.integers(0, ng, m)], "s": s[rng.integers(0, ns, m)], "f": np.full(m, f),
+               "v0": rng.integers(0, 100, m)})
+    t.extents(v0=(0, 100))
+    sp = t.spec
+    word = r"hashed=1 hashg=0 gbits=31 fbits=1 tbit=0 "
+    qs = [_q(sp, int_filters=[("f", "eq", 1)], groups=["g", "s"], aggs=["v0"], op="avg",
+             expect=[r"fail_mode=1 .*nslots=65536 " + word]),
+          _q(sp, int_filters=[("f", "eq", 2)], groups=["g", "s"], aggs=[], op="avg",
+             expect=[r"nslots=65536 " + word]),
+          _q(sp, int_filters=[("f", "eq", 3)], groups=["s", "g"], aggs=[], op="avg",
+             expect=[r"nslots=131072 " + word])]
+    qs[0].wraps = pick  # (ig, is) of the keys whose probe chains wrap, for the test that checks they are there
+    return t.done(qs)
+
+
+def i_refused(spec):
+    """Queries the planner must refuse on the ceiling table: the 2^31 - 2 codes with a time bit (33 bits), and a
+    product past 2^31 - 2."""
+    return [_q(spec, int_filters=[("f", "eq", 1)], groups=["g", "s"], aggs=[], op="avg", time_col="f",
+               time_bucket=1),
+            _q(spec, int_filters=[("f", "eq", 1)], groups=["g", "s2"], aggs=[], op="avg")]
+
+
+KEY_TABLES = {"G-int": lambda forms=None: family_g_int(False, forms),
+              "G-mixed": lambda forms=None: family_g_int(True, forms),
+              "G-str": family_g_str, "H": family_h, "K": family_k,
+              "I-dense": lambda forms=None: family_i_dense(False, forms),
+              "I-hashed": lambda forms=None: family_i_dense(True, forms), "I-ceiling": family_i_ceiling}
+
+
 def all_tables(forms=None):
     """(name, (spec, rows, valid, queries)) of every family."""
     out = [("A", family_a(forms))]
@@ -329,4 +655,5 @@ def all_tables(forms=None):
     out += [("C%d" % i, x) for i, x in enumerate(family_c(forms))]
     out += [("D%d" % i, x) for i, x in enumerate(family_d(forms))]
     out += [("E", family_e(forms)), ("F", family_f(forms))]
+    out += [(name, build(forms)) for name, build in KEY_TABLES.items()]
     return out

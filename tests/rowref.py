@@ -11,7 +11,7 @@ result is adopted first (Q9) and stay compared against the oracle through `tests
 their validity masks ({name: bool array}; an absent name is fully valid)."""
 import numpy as np
 
-from tests.util import INT, STR
+from tests.util import INT, SET, STR
 
 NUM_BUCKETS = 1000  # hist.go:3
 I64_MIN, I64_MAX = -(1 << 63), (1 << 63) - 1
@@ -144,7 +144,21 @@ def decode(n, typ, vals, va, threshold):
     """What a block's column file holds once read back (column_store_io.go:82-113 writes it, :493-609,690-780 read
     it): (values, populated) over the block's n rows, or None when no row has the column (no file is written).
     Few distinct values: one bin per value, only the listed rows are populated.  Many: a Values array up to the
-    last valid row, whose gaps read int 0 or string id 0 — the block's first string."""
+    last valid row, whose gaps read int 0 or string id 0 — the block's first string.
+    A set column (SaveSetsToColumns, column_store_io.go:139-217; unpackSetCol :611-688): (per-row tag sets,
+    populated).  Without any tag in the block no file is written.  Few distinct tags: bins, so a row is populated
+    when its set is not empty.  Many: Values [][]int32 up to the last row holding a tag, every row below populated."""
+    if typ == SET:
+        tags = [frozenset(str(x) for x in s) if ok else frozenset() for s, ok in zip(vals, va)]
+        held = [r for r, s in enumerate(tags) if s]
+        if not held:
+            return None
+        pop = np.array([bool(s) for s in tags])
+        if len(set().union(*tags)) > threshold:
+            pop[:held[-1] + 1] = True
+        out = np.empty(n, object)
+        out[:] = tags
+        return out, pop
     idx = np.nonzero(va)[0]
     if not len(idx):
         return None
@@ -240,6 +254,12 @@ def run(spec, rows, valid, q):
                 for c, op, v in q.str_filters:  # filter.go:199-250 on the decoded string
                     xv, xp = cv.get(c, empty)
                     if not (xp[i] and ((xv[i] == v) if op == "eq" else (xv[i] != v))):
+                        ok = False
+                        break
+            if ok:
+                for c, op, v in q.set_filters:  # filter.go:252-285: a row without a set fails in and nin
+                    xv, xp = cv.get(c, empty)
+                    if not (xp[i] and ((v in xv[i]) if op == "in" else (v not in xv[i]))):
                         ok = False
                         break
             if not ok:
@@ -338,10 +358,29 @@ def check(ref, got, q, hists_of=lambda g: g.Hists, where=""):
                                                    [(k, x, y) for k, (x, y) in enumerate(zip(vals, rvals)) if x != y][:8])
 
     assert got.MatchedCount == ref.MatchedCount, (where, "MatchedCount", got.MatchedCount, ref.MatchedCount)
-    assert set(got.Results) == set(ref.Results), (where, "group keys",
-                                                  sorted(set(got.Results) ^ set(ref.Results))[:8])
-    for k, rg in ref.Results.items():
-        grp(rg, got.Results[k], (where, "Results", k))
+    # Results is a dict keyed by the rendered key: two groups with one key would hide each other there, so the
+    # group counts are checked on the lists the dicts were built from
+    if hasattr(got, "NumGroups"):
+        assert got.NumGroups == len(ref.Results), (where, "NumGroups", got.NumGroups, len(ref.Results))
+    keys = [r.GroupByKey for r in getattr(got, "Sorted", None) or got.Results.values()]
+    assert len(keys) == len(set(keys)), (where, "groups sharing a key", sorted(k for k in set(keys)
+                                                                                if keys.count(k) > 1)[:8])
+    if q.limit:  # the first `limit` groups by Count descending; the tables keep the cut tie-free
+        order = sorted(ref.Results, key=lambda k: (-ref.Results[k].Count, k))
+        want = order[:q.limit]
+        if len(order) > q.limit:
+            assert ref.Results[order[q.limit - 1]].Count != ref.Results[order[q.limit]].Count, (where, "tie at the cut")
+        if hasattr(got, "NumGroups"):  # the engine materialises exactly the first `limit` groups
+            assert len(keys) == len(want), (where, "groups under limit", len(keys), len(want))
+        if hasattr(got, "Sorted"):
+            assert keys[:q.limit] == want, (where, "top groups", keys[:8], want[:8])
+        else:
+            assert set(want) <= set(keys), (where, "top groups")
+    else:
+        assert set(got.Results) == set(ref.Results), (where, "group keys",
+                                                      sorted(set(got.Results) ^ set(ref.Results))[:8])
+    for k in got.Results:
+        grp(ref.Results[k], got.Results[k], (where, "Results", k))
     if q.time_col:
         assert (got.Cumulative.Count, got.Cumulative.Samples) == (ref.Cumulative.Count, ref.Cumulative.Samples)
     else:
@@ -349,6 +388,8 @@ def check(ref, got, q, hists_of=lambda g: g.Hists, where=""):
     assert set(got.TimeResults) == set(ref.TimeResults), (where, "time buckets",
                                                           sorted(set(got.TimeResults) ^ set(ref.TimeResults))[:8])
     for tb, m in ref.TimeResults.items():
+        n = getattr(got, "TimeNumGroups", {}).get(tb, len(got.TimeResults[tb]))
+        assert n == len(m), (where, "time groups", tb, "groups sharing a key")
         assert set(got.TimeResults[tb]) == set(m), (where, "time groups", tb)
         for k, rg in m.items():
             grp(rg, got.TimeResults[tb][k], (where, "TimeResults", tb, k))
