@@ -367,8 +367,10 @@ struct sg_table {
   std::vector<uint32_t> pending_stats;  // value-array int columns whose extents are not computed yet
   // sort ranks of the dictionaries' rendered fields (ties of SortResults break by GroupByKey ascending):
   // rank[id] over the strings (resp. the decimal renderings of the int values) + '\t'; rebuilt when a
-  // dictionary has grown
+  // dictionary has grown.  splain[col]: no string of srank[col]'s dictionary holds a byte <= '\t' (the ranks
+  // then give GroupByKey order field by field)
   std::vector<std::vector<uint32_t>> srank, irank;
+  std::vector<uint8_t> splain;
   std::vector<std::pair<char*, size_t>> chunks;  // device arena chunks (ptr, capacity)
   size_t chunk_idx = 0, chunk_used = 0;
   Stage stage[2];
@@ -612,6 +614,7 @@ sg_table* sg_table_create(sg_ctx* c, int32_t num_col_slots, const int32_t* col_t
   t->iseed.assign((size_t)num_col_slots, -1);
   t->srank.assign((size_t)num_col_slots, std::vector<uint32_t>());
   t->irank.assign((size_t)num_col_slots, std::vector<uint32_t>());
+  t->splain.assign((size_t)num_col_slots, 1);
   cudaSetDevice(c->device);
   for (int i = 0; i < 2; i++) {
     if (cudaHostAlloc((void**)&t->stage[i].host, STAGE_BYTES, cudaHostAllocDefault) != cudaSuccess ||
@@ -2489,28 +2492,30 @@ void sort_groups(const sg_query* q, std::vector<ResultGroup>& v) {
   if (q->d.order_asc) std::reverse(v.begin(), v.end());
 }
 
-// a < b for the rendered fields a + '\t', b + '\t'
-static inline bool tab_less(const std::string& a, const std::string& b) {
-  const size_t n = std::min(a.size(), b.size());
-  const int c = memcmp(a.data(), b.data(), n);
-  if (c != 0) return c < 0;
-  if (a.size() == b.size()) return false;
-  return a.size() < b.size() ? (unsigned char)'\t' < (unsigned char)b[n] : (unsigned char)a[n] < (unsigned char)'\t';
-}
-static void ranks_of(const std::vector<std::string>& strs, std::vector<uint32_t>& rank) {
+// Ties of SortResults break by the rendered GroupByKey, the fields joined with '\t', compared as bytes.  When no
+// string of an axis holds a byte <= '\t', the order of its fields f + '\t' is the byte order of the strings, the
+// missing field ("") comes first, and comparing whole keys is comparing field by field: a per-axis rank gives
+// the order.  Otherwise ("\x01" sorts before missing; "a\tb" against "a" depends on the next field) the keys
+// themselves are compared (slot_key).
+static bool ranks_of(const std::vector<std::string>& strs, std::vector<uint32_t>& rank) {
+  bool plain = true;
+  for (const auto& s : strs)
+    for (unsigned char ch : s) plain = plain && ch > (unsigned char)'\t';
   std::vector<uint32_t> idx(strs.size());
   for (size_t i = 0; i < idx.size(); i++) idx[i] = (uint32_t)i;
-  std::sort(idx.begin(), idx.end(), [&](uint32_t x, uint32_t y) { return tab_less(strs[x], strs[y]); });
+  std::sort(idx.begin(), idx.end(), [&](uint32_t x, uint32_t y) { return strs[x] < strs[y]; });
   rank.resize(strs.size());
   for (size_t i = 0; i < idx.size(); i++) rank[idx[i]] = (uint32_t)i;
+  return plain;
 }
-// rank of every code of one slot-space axis in the order of its rendered field (code 0 = missing = "" first)
-static const std::vector<uint32_t>& axis_ranks(sg_query* q, size_t di, std::vector<uint32_t>& scratch) {
+// rank of every code of one slot-space axis in the order of its rendered field (code 0 = missing = "" first);
+// *plain is cleared when the ranks do not give that order (a string holds a byte <= '\t')
+static const std::vector<uint32_t>& axis_ranks(sg_query* q, size_t di, std::vector<uint32_t>& scratch, bool* plain) {
   const GroupDim& d = q->dims[di];
   sg_table* t = q->table;
   if (q->merged) {  // union dictionaries of a cross-GPU merge: per query
     if (d.is_str) {
-      ranks_of(q->m_strs[di], scratch);
+      if (!ranks_of(q->m_strs[di], scratch)) *plain = false;
     } else {
       std::vector<std::string> r;
       for (int64_t v : q->m_ints[di]) r.push_back(std::to_string(v));
@@ -2519,12 +2524,14 @@ static const std::vector<uint32_t>& axis_ranks(sg_query* q, size_t di, std::vect
     return scratch;
   }
   if (d.is_str && q->repl.count(d.col)) {
-    ranks_of(q->repl.at(d.col).strs, scratch);
+    if (!ranks_of(q->repl.at(d.col).strs, scratch)) *plain = false;
     return scratch;
   }
   if (d.is_str) {
     auto& cache = t->srank[(size_t)d.col];
-    if (cache.size() != t->sdict[(size_t)d.col].strs.size()) ranks_of(t->sdict[(size_t)d.col].strs, cache);
+    if (cache.size() != t->sdict[(size_t)d.col].strs.size())
+      t->splain[(size_t)d.col] = ranks_of(t->sdict[(size_t)d.col].strs, cache) ? 1 : 0;
+    if (!t->splain[(size_t)d.col]) *plain = false;
     return cache;
   }
   auto& cache = t->irank[(size_t)d.col];
@@ -2566,6 +2573,12 @@ static void group_key(const sg_query* q, uint32_t s, ResultGroup& g, int64_t* tb
       g.key.push_back((uint64_t)q->table->idict[(size_t)d.col].vals[code - 1]);
   }
   g.skey = render_key(q, g.key);
+}
+// the rendered GroupByKey of slot s (ties between keys whose fields hold bytes <= '\t', axis_ranks)
+static std::string slot_key(const sg_query* q, uint32_t s) {
+  ResultGroup g;
+  group_key(q, s, g, nullptr);
+  return std::move(g.skey);
 }
 static void make_group(const sg_query* q, const uint64_t* h, uint32_t s, ResultGroup& g, int64_t* tbucket,
                        const std::vector<uint64_t>* samples = nullptr) {
@@ -2611,8 +2624,9 @@ static void parallel_slots(uint32_t n, int want, Fn fn) {
 // keys (11 bits a pass, from the top set bit down) to the key of the limit-th group, then every slot at or above
 // it with its values — instead of reading a 40 MB accumulator array back and scanning a million slots on the
 // host.  Ties at the cut are all emitted and broken on the host exactly as sort_groups does.
-// Returns SG_OK with *out set, 1 when the query is not of that shape (or the tie group is huge): host path.
-static int build_result_topk(sg_query* q, sg_result** out) {
+// Returns SG_OK with *out set, 1 when the query is not of that shape (or the tie group is huge, *fell_back set):
+// host path.
+static int build_result_topk(sg_query* q, sg_result** out, bool* fell_back) {
   sg_ctx* c = q->ctx;
   const Plan& P = q->plan;
   const int naggs = P.naggs, ob = q->d.order_by_agg;
@@ -2700,7 +2714,10 @@ static int build_result_topk(sg_query* q, sg_result** out) {
   CUDA_TRY(c, cudaStreamSynchronize(c->stream));
   q->launches += 1;
   T = *(const TopkTotals*)(hp + off_tot);
-  if (T.overflow || T.n_out > cap) return 1;  // a huge group of ties at the cut: the host path sorts them all
+  if (T.overflow || T.n_out > cap) {  // a huge group of ties at the cut: the host path sorts them all
+    *fell_back = true;
+    return 1;
+  }
   const size_t n = T.n_out;
   CUDA_TRY(c, cudaMemcpyAsync(hp + off_rows, d_rows, n * w * 8, cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(c, cudaStreamSynchronize(c->stream));
@@ -2708,16 +2725,19 @@ static int build_result_topk(sg_query* q, sg_result** out) {
   const unsigned long long* rows = (const unsigned long long*)(hp + off_rows);
   const uint64_t* scal = (const uint64_t*)(hp + off_scal);
 
-  // exact order of the candidates: value descending, ties by GroupByKey ascending (ranks of the rendered fields)
+  // exact order of the candidates: value descending, ties by GroupByKey ascending (ranks of the rendered fields,
+  // or the keys themselves when the ranks do not give that order)
   std::vector<std::vector<uint32_t>> scratch(q->dims.size());
   std::vector<const std::vector<uint32_t>*> ranks(q->dims.size(), nullptr);
-  for (size_t di = 0; di < q->dims.size(); di++) ranks[di] = &axis_ranks(q, di, scratch[di]);
+  bool plain = true;
+  for (size_t di = 0; di < q->dims.size(); di++) ranks[di] = &axis_ranks(q, di, scratch[di], &plain);
   struct Ent {
     double v;
     uint64_t tie;
     uint32_t row;
   };
   std::vector<Ent> ents(n);
+  std::vector<std::string> keys(plain ? 0 : n);
   for (size_t i = 0; i < n; i++) {
     const unsigned long long* r = rows + i * w;
     const uint32_t sl = (uint32_t)r[0];
@@ -2730,8 +2750,12 @@ static int build_result_topk(sg_query* q, sg_result** out) {
     ents[i].v = order_value(q, (int64_t)r[1], ob >= 0 ? (int64_t)r[2 + 2 * ob] : 0, ob >= 0 ? (int64_t)r[3 + 2 * ob] : 0);
     ents[i].tie = tie;
     ents[i].row = (uint32_t)i;
+    if (!plain) keys[i] = slot_key(q, sl);
   }
-  std::sort(ents.begin(), ents.end(), [](const Ent& a, const Ent& b) { return a.v != b.v ? a.v > b.v : a.tie < b.tie; });
+  std::sort(ents.begin(), ents.end(), [&](const Ent& a, const Ent& b) {
+    if (a.v != b.v) return a.v > b.v;
+    return plain ? a.tie < b.tie : keys[a.row] < keys[b.row];
+  });
   if ((int64_t)ents.size() > limit) ents.resize((size_t)limit);
 
   std::unique_ptr<sg_result> r(new sg_result());
@@ -2866,9 +2890,16 @@ static int fold_axes(sg_query* q, uint64_t* h, size_t have, sg_result* r, int64_
 int build_result(sg_query* q, sg_result** out) {
   sg_ctx* c = q->ctx;
   const Plan& P = q->plan;
+  // SG_PLAN_TRACE=1: which selection built the result ("sg_select: path=device|device-fallback|host threads=N")
+  // (device-fallback: the device found more ties at the cut than it keeps, and the host selected)
+  const bool trace = getenv("SG_PLAN_TRACE") != nullptr;
+  bool fell_back = false;
   {
-    const int rc = build_result_topk(q, out);
-    if (rc != 1) return rc;
+    const int rc = build_result_topk(q, out, &fell_back);
+    if (rc != 1) {
+      if (trace && rc == SG_OK) fprintf(stderr, "sg_select: path=device threads=1\n");
+      return rc;
+    }
   }
   const bool time_mode = P.time_col >= 0;
   const int naggs = P.naggs;
@@ -2945,6 +2976,11 @@ int build_result(sg_query* q, sg_result** out) {
   for (int i = 1; i < (int)q->groups.size(); i++) r->total.skey += "\t";
   r->has_total_hists = !time_mode;
   const uint64_t* cnt = h + q->off_count;
+  // a group is a slot that rows were scanned into.  Weighted, its Count is the sum of the rows' weights and can
+  // be 0 (weight 0, +w / -w, wrapped): the rows per slot (r->samples) decide then, as in the reference, where
+  // every row creates its group (aggregate.go:156-203)
+  const uint64_t* rows_of = r->samples.empty() ? cnt : (const uint64_t*)r->samples.data();
+  const bool weighted = !r->samples.empty();
 
   if (!time_mode) {
     // ---- lazy result: live slots, Cumulative, order -------------------------------------------------
@@ -2952,12 +2988,15 @@ int build_result(sg_query* q, sg_result** out) {
     const int ob = q->d.order_by_agg;
     const int64_t limit = q->d.limit;
     int hw = (int)std::thread::hardware_concurrency();
-    const int nt = std::max(1, std::min(hw > 0 ? hw : 1, 16));
-    // tie-break ranks: GroupByKey ascending == lexicographic over the axes' rendered fields
+    int nt = std::max(1, std::min(hw > 0 ? hw : 1, 16));
+    if (const char* e = getenv("SG_HOST_THREADS")) nt = std::max(1, std::min(atoi(e), 16));  // tests: 1 vs many
+    // tie-break ranks: GroupByKey ascending == lexicographic over the axes' rendered fields, when `plain`;
+    // otherwise tied entries compare their rendered keys
     std::vector<std::vector<uint32_t>> scratch(q->dims.size());
     std::vector<const std::vector<uint32_t>*> ranks(q->dims.size(), nullptr);
+    bool plain = true;
     if (ob != SG_ORDER_NONE)
-      for (size_t di = 0; di < q->dims.size(); di++) ranks[di] = &axis_ranks(q, di, scratch[di]);
+      for (size_t di = 0; di < q->dims.size(); di++) ranks[di] = &axis_ranks(q, di, scratch[di], &plain);
     auto tie_of = [&](uint32_t s) {
       uint64_t tie = 0;
       const uint32_t cs = slot_code(q, s);
@@ -2973,7 +3012,10 @@ int build_result(sg_query* q, sg_result** out) {
       uint64_t tie;
       uint32_t slot;
     };
-    auto before = [](const Ent& a, const Ent& b) { return a.v != b.v ? a.v > b.v : a.tie < b.tie; };
+    auto before = [&](const Ent& a, const Ent& b) {
+      if (a.v != b.v) return a.v > b.v;
+      return plain ? a.tie < b.tie : slot_key(q, a.slot) < slot_key(q, b.slot);
+    };
     struct Part {
       std::vector<Ent> ents;
       ResultGroup tot;
@@ -2991,14 +3033,14 @@ int build_result(sg_query* q, sg_result** out) {
         for (int a = 0; a < naggs; a++) p.tot.values[(size_t)a].assign(q->layouts[(size_t)a].nvals_total, 0);
       }
       for (uint32_t s = s0; s < s1; s++) {
+        if (rows_of[s] == 0) continue;
         const int64_t n = (int64_t)cnt[s];
-        if (n == 0) continue;
         p.live++;
         p.tot.count += n;
         int64_t hc_o = 0, sm_o = 0;
         for (int a = 0; a < naggs; a++) {
           const int64_t hc = q->hc_is_count[(size_t)a] ? n : (int64_t)h[q->off_hcount[(size_t)a] + s];
-          if (hc == 0) continue;
+          if (hc == 0 && !weighted) continue;  // (weighted, a histogram whose Count folds to 0 still has a sum)
           const int64_t sm = (int64_t)h[q->off_sum[(size_t)a] + s];
           p.tot.hc(a) += hc;
           p.tot.sm(a) = (int64_t)((uint64_t)p.tot.sm(a) + (uint64_t)sm);
@@ -3066,6 +3108,8 @@ int build_result(sg_query* q, sg_result** out) {
     if (w_rows >= 0) r->total.samples = w_rows;
     r->lazy = true;
     r->acc_have = have;
+    if (trace)
+      fprintf(stderr, "sg_select: path=%s threads=%d\n", fell_back ? "device-fallback" : "host", ns >= (1u << 17) ? nt : 1);
     if (!r->pin) {
       r->acc.swap(hv);
       r->accp = r->acc.data();
@@ -3080,7 +3124,7 @@ int build_result(sg_query* q, sg_result** out) {
   std::map<std::vector<uint64_t>, size_t> by_key;                    // Results in time mode
   std::map<int64_t, std::unique_ptr<sg_result>> slices;              // TimeResults
   for (uint32_t s = 0; s < P.nslots; s++) {
-    if (cnt[s] == 0) continue;
+    if (rows_of[s] == 0) continue;
     ResultGroup g;
     int64_t tbucket = 0;
     make_group(q, h, s, g, &tbucket, r->samples.empty() ? nullptr : &r->samples);
@@ -3123,6 +3167,7 @@ int build_result(sg_query* q, sg_result** out) {
     r->time_keys.push_back(kv.first);
     r->time_slices.push_back(std::move(kv.second));
   }
+  if (trace) fprintf(stderr, "sg_select: path=host threads=1\n");
   *out = r.release();
   return SG_OK;
 }

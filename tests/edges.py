@@ -641,6 +641,228 @@ def i_refused(spec):
             _q(spec, int_filters=[("f", "eq", 1)], groups=["g", "s2"], aggs=[], op="avg")]
 
 
+# ---------------------------------------------------------------------------------------------------------------
+# L, W, R. Result shaping: order, limit and ties; weights; StrReplace
+# ---------------------------------------------------------------------------------------------------------------
+# Every query of these families carries `expect` patterns for its `sg_select:` trace line (build_result's choice
+# of selection path).  Ties break by the rendered GroupByKey as bytes: a leading byte below '\t' sorts before the
+# missing field, an embedded tab compares against the next field's bytes.
+KT_ORDER = [("s", STR), ("s2", STR), ("k", INT), ("k2", INT), ("t", INT), ("w", INT), ("f", INT), ("v0", INT),
+            ("v1", INT)]
+V0_HI = I64_MAX // 10  # 10 * V0_HI = INT64_MAX - 7: values up to there are accepted
+# str key, rows, v0 values, v1 values (the other rows lack the column).  Counts tie on purpose: six groups of 6
+# (missing, the control-byte and the tab keys), four of 3, two of 2.  Means: 1/3 and 2/6, -7.5 twice, 2^53 and
+# 2^53 + 1 (one double), INT64_MAX - 7 twice (the sum wraps to -16), and no v0 / v1 histogram on many groups
+L_STR = [(None, 6, [1, 0, 0], [5]),
+         ("\x01", 6, [1, 1, 0, 0, 0, 0], []),
+         ("\x08z", 6, [-7, -8], [5]),
+         ("a\tb", 6, [1 << 53], [-3]),
+         ("a", 6, [(1 << 53) + 1], []),
+         ("\t", 6, [], [5]),
+         ("a\tc", 3, [V0_HI * 10, V0_HI * 10], []),
+         ("é", 3, [-8, -7], []),
+         ("日本", 3, [], []),
+         ("z", 3, [], [-1]),
+         ("b", 2, [], []),
+         ("c", 2, [1, 2], [])]
+L_INT = [9, 10, -5, I64_MIN, -1, 100]  # -1 renders (and groups) as missing
+
+
+def _sel(path, threads=None):
+    return [r"^sg_select: path=%s threads=%s$" % (path, threads if threads is not None else r"\d+")]
+
+
+def _l_rows(t, block_split=True):
+    """The L_STR groups as rows: k cycles over L_INT and the missing value, t over two time buckets."""
+    s, sv, v0, v0v, v1, v1v = [], [], [], [], [], []
+    for key, n, a, b in L_STR:
+        for i in range(n):
+            s.append(key or "")
+            sv.append(key is not None)
+            v0.append(a[i] if i < len(a) else 0)
+            v0v.append(i < len(a))
+            v1.append(b[i] if i < len(b) else 0)
+            v1v.append(i < len(b))
+    n = len(s)
+    kk = [L_INT[i % 7] if i % 7 < len(L_INT) else 0 for i in range(n)]
+    cols = {"s": np.asarray(s, dtype=object).astype(str), "k": kk, "t": [(i * 37) % 2000 for i in range(n)],
+            "v0": v0, "v1": v1}
+    valid = {"s": np.asarray(sv), "k": np.asarray([i % 7 < len(L_INT) for i in range(n)]),
+             "v0": np.asarray(v0v), "v1": np.asarray(v1v)}
+    # first half bucket-encoded, second half as value arrays
+    h = n // 2
+    t.add({c: v[:h] for c, v in cols.items()}, {c: v[:h] for c, v in valid.items()})
+    t.add({c: v[h:] for c, v in cols.items()}, {c: v[h:] for c, v in valid.items()}, threshold=2)
+
+
+def _live(spec, rows, valid, q):
+    from tests import rowref
+    return len(rowref.run(spec, rows, valid, q).Results)
+
+
+def _l_queries(t, groups_list, limits_of, orders=("$COUNT", "v0", "v1"), time=False, expect=None):
+    s = t.spec
+    qs = []
+    for groups in groups_list:
+        live = _live(s, t.rows, t.valid, Q(s, groups=groups, aggs=["v0", "v1"], op="avg"))
+        for ob in orders:
+            for asc in (False, True):
+                for limit in limits_of(live):
+                    kw = dict(time_col="t", time_bucket=1000) if time else {}
+                    qs.append(_q(s, groups=groups, aggs=["v0", "v1"], op="avg", order_by=ob, order_asc=asc,
+                                 limit=limit, expect=expect(ob, asc, limit, live) if expect else _sel("host", 1),
+                                 **kw))
+        for limit in (0, 2):  # OrderBy "": any `limit` groups
+            qs.append(_q(s, groups=groups, aggs=["v0", "v1"], op="avg", order_by="", limit=limit,
+                         expect=_sel("host", 1)))
+    return qs
+
+
+def family_l_small(forms=None):
+    """Fewer than 2^17 slots: the lazy host path on one thread, and time mode."""
+    t = _Table(forms, KT_ORDER)
+    _l_rows(t)
+    t.extents(v0=(-(1 << 62), V0_HI), v1=(-100, 100))
+    qs = _l_queries(t, [["s"], ["k"], ["s", "k"], ["k", "s"]], lambda live: (0, 1, 3, live - 1, live, live + 1))
+    qs += _l_queries(t, [["s"], ["s", "k"]], lambda live: (0, 3), time=True)
+    return t.done(qs)
+
+
+L_LIMIT = 100  # the device path's cap is L_LIMIT + 8192 candidates
+L_TIED = L_LIMIT + 8192 - (L_LIMIT - 1)  # groups tied at the cut that fill the cap exactly
+
+
+def family_l_large(forms=None):
+    """More than 2^17 slots (s: 64 codes x k2: 5,000) with accumulators too large to come back behind the scan:
+    the device top-K, its fall-back to the host and the host's many-thread selection.  L_LIMIT - 1 groups of 3
+    rows, L_TIED + 1 groups of 2 (the last one's rows have f = 1: without them the candidates at the cut number
+    L_LIMIT + 8192 exactly, with them one more) and filler groups of 1 row.  The groups of 2 include every
+    control-byte, tab and missing key, so which of them make the cut depends on full-key byte order."""
+    rng = np.random.default_rng(40)
+    t = _Table(forms, KT_ORDER)
+    strs = [k for k, _, _, _ in L_STR if k is not None] + ["s%02d" % i for i in range(51)]  # 63 strings + missing
+    n3, n2, n1 = L_LIMIT - 1, L_TIED + 1, 2000
+    tied = [(a, b) for a in [None] + strs[:12] for b in range(5)]  # control / tab / missing keys among the tied
+    others = [(a, b) for b in range(5, 4999) for a in [None] + strs]  # every other (s, k2) group
+    sel = [others[i] for i in rng.permutation(len(others))[:n3 + n2 - len(tied) + n1]]
+    top, tied, filler = sel[:n3], tied + sel[n3:n3 + n2 - len(tied)], sel[n3 + n2 - len(tied):]
+    groups = [(p, 3, 0) for p in top] + [(p, 2, 0) for p in tied[:-1]] + [(tied[-1], 2, 1)] + [(p, 1, 0) for p in filler]
+    rows = [(p, f) for p, c, f in groups for _ in range(c)]
+    rows = [rows[i] for i in rng.permutation(len(rows))]
+    n = len(rows)
+    cols = {"s": np.asarray([p[0] or "" for p, _ in rows]), "k2": [p[1] for p, _ in rows],
+            "f": [f for _, f in rows], "t": rng.integers(0, 2000, n),
+            "v0": rng.integers(-50, 50, n), "v1": rng.integers(-5, 5, n)}
+    cols["v0"][:4] = [1 << 53, (1 << 53) + 1, V0_HI * 10, -7]
+    valid = {"s": np.asarray([p[0] is not None for p, _ in rows]), "v1": rng.random(n) < 0.3}
+    t.add(cols, valid, block_rows=8192)
+    t.extents(v0=(-(1 << 62), V0_HI), v1=(-100, 100))
+    s = t.spec
+    big = dict(groups=["s", "k2"], aggs=["v0", "v1"], op="avg")
+    cap = [("f", "neq", 1)]
+    qs = [_q(s, int_filters=cap, order_by="$COUNT", limit=L_LIMIT, expect=_sel("device", 1), **big),
+          _q(s, order_by="$COUNT", limit=L_LIMIT, expect=_sel("device-fallback"), **big)]
+    live = len(groups)
+
+    def expect(ob, asc, limit, live):
+        return _sel("device", 1) if not asc and 1 <= limit <= 65536 else _sel("host")
+    for ob in ("$COUNT", "v0", "v1"):
+        for asc in (False, True):
+            for limit in (1, live - 1, live, live + 1, 65536, 65537):
+                qs.append(_q(s, order_by=ob, order_asc=asc, limit=limit, expect=expect(ob, asc, limit, live), **big))
+    qs.append(_q(s, order_by="", limit=3, expect=_sel("host"), **big))
+    qs.append(_q(s, order_by="$COUNT", limit=5, time_col="t", time_bucket=1000, expect=_sel("host", 1), **big))
+    for q in qs:
+        q.live = live
+    return t.done(qs)
+
+
+def family_w(forms=None):
+    """Weights: 0, -1 (a weight, not the missing alias), negative, +w / -w pairs in one group, 2^62 x 4 rows (Count
+    wraps to 0), values next to INT64_MAX.  Groups made only of weight-0 rows; the weight column bucket-encoded in
+    one block and a value array in the other."""
+    t = _Table(forms, KT_ORDER)
+    groups = [("zero", [0, 0, 0]), ("neg1", [-1, -1]), ("neg", [-5, -5, 3]), ("cancel", [7, -7]),
+              ("wrap", [1 << 62] * 4), ("big", [I64_MAX, 1]), ("max", [I64_MAX - 1]), ("plain", [1, 2, 3]),
+              (None, [2, 0]), ("zero2", [0]), ("one", [1])]
+    s, sv, w, v0 = [], [], [], []
+    for key, ws in groups:
+        for i, x in enumerate(ws):
+            s.append(key or "")
+            sv.append(key is not None)
+            w.append(x)
+            v0.append((len(s) * 13) % 101)
+    n = len(s)
+    for thr in (5000, 3):
+        t.add({"s": s, "w": w, "t": [(i * 211) % 1500 for i in range(n)], "v0": v0, "v1": v0[::-1]},
+              {"s": np.asarray(sv), "v1": np.arange(n) % 3 > 0}, threshold=thr)
+    t.extents(v0=(0, 100), v1=(0, 100))
+    sp = t.spec
+    qs = []
+    for op, loghist in (("avg", False), ("hist", False), ("avg", True)):
+        for time in (False, True):
+            kw = dict(time_col="t", time_bucket=500) if time else {}
+            for ob, limit in (("$COUNT", 0), ("v0", 0), ("v1", 4), ("$COUNT", 3)):
+                qs.append(_q(sp, groups=["s"], aggs=["v0", "v1"], op=op, loghist=loghist, weight_col="w",
+                             order_by=ob, limit=limit, expect=_sel("host", 1), **kw))
+    for q in qs:
+        # the reference drops a block's group result whose Count is 0 when it combines blocks, unless that block
+        # is the first to hold the group (query_spec.go:143-145, DESIGN.md §7); the oracle and pyoracle restate that
+        q.oracle = q.pyoracle = False
+    return t.done(qs)
+
+
+def family_r(forms=None):
+    """StrReplace with order and limit: merging rewrites whose merged groups decide the cut, rewrites to "" and
+    to strings with a leading control byte or a tab, rewrites on both group columns, a rewrite with weights, and
+    a filter on the rewritten column."""
+    t = _Table(forms, KT_ORDER)
+    # s: ab1..ab4 merge into "ab" (4 groups of 2 rows -> one of 8, above every other group), cd -> "\x01c",
+    # xy -> "\tx", zz -> "" (the missing group)
+    counts = {"ab1": 2, "ab2": 2, "ab3": 2, "ab4": 2, "ab": 1, "cd": 5, "xy": 5, "zz": 3, "m": 5, "n": 6, None: 2}
+    s = [k for k, c in counts.items() for _ in range(c)]
+    n = len(s)
+    s2 = ["q%d" % (i % 3) if i % 4 else "r" for i in range(n)]
+    cols = {"s": np.asarray([x or "" for x in s]), "s2": np.asarray(s2), "w": [1 + i % 3 for i in range(n)],
+            "t": [(i * 97) % 1000 for i in range(n)], "v0": [(i * 7) % 50 for i in range(n)]}
+    valid = {"s": np.asarray([x is not None for x in s])}
+    t.add({c: v[:n // 2] for c, v in cols.items()}, {c: v[:n // 2] for c, v in valid.items()})
+    t.add({c: v[n // 2:] for c, v in cols.items()}, {c: v[n // 2:] for c, v in valid.items()}, threshold=3)
+    t.extents(v0=(0, 50))
+    sp = t.spec
+    merge = {"s": (r"^(ab)\d$", "$1")}
+    ctrl = {"s": (r"^cd$", "\x01c")}
+    tab = {"s": (r"^x(y)$", "\t$1")}
+    empty = {"s": (r"^zz$", "")}
+    both = {"s": (r"^(ab)\d$", "$1"), "s2": (r"^q\d$", "q")}
+    allr = {**merge, **ctrl, **tab, **empty}
+    qs = []
+    for rep in (merge, ctrl, tab, empty, both, allr):
+        for ob, asc, limit in (("$COUNT", False, 1), ("$COUNT", False, 3), ("$COUNT", True, 2), ("v0", False, 3),
+                               ("$COUNT", False, 0), ("", False, 2)):
+            groups = ["s", "s2"] if rep is both else ["s"]
+            q = _q(sp, groups=groups, aggs=["v0"], op="avg", order_by=ob, order_asc=asc, limit=limit,
+                   str_replace=rep, expect=_sel("host", 1))
+            # the C++ oracle keeps one of "" and missing (family_g_str): not compared under rewrites to ""
+            q.oracle = rep is not empty and rep is not allr
+            qs.append(q)
+    qs.append(_q(sp, groups=["s"], aggs=["v0"], op="hist", weight_col="w", order_by="$COUNT", limit=3,
+                 str_replace=merge, expect=_sel("host", 1)))
+    qs.append(_q(sp, groups=["s"], aggs=["v0"], op="avg", order_by="$COUNT", limit=2, time_col="t", time_bucket=500,
+                 str_replace=allr, expect=_sel("host", 1)))
+    qs[-1].oracle = False
+    # a filter on the rewritten column: "ab" is a present literal, but under the merging rewrite the reference's
+    # lookup maps it to one of the merged ids (DESIGN.md §7), so the oracle is not compared
+    q = _q(sp, str_filters=[("s", "eq", "ab")], groups=["s", "s2"], aggs=["v0"], op="avg", order_by="$COUNT",
+           limit=2, str_replace=merge, expect=_sel("host", 1))
+    q.oracle = False
+    qs.append(q)
+    return t.done(qs)
+
+
+ORDER_TABLES = {"L-small": family_l_small, "L-large": family_l_large, "W": family_w, "R": family_r}
+
+
 KEY_TABLES = {"G-int": lambda forms=None: family_g_int(False, forms),
               "G-mixed": lambda forms=None: family_g_int(True, forms),
               "G-str": family_g_str, "H": family_h, "K": family_k,
@@ -656,4 +878,5 @@ def all_tables(forms=None):
     out += [("D%d" % i, x) for i, x in enumerate(family_d(forms))]
     out += [("E", family_e(forms)), ("F", family_f(forms))]
     out += [(name, build(forms)) for name, build in KEY_TABLES.items()]
+    out += [(name, build(forms)) for name, build in ORDER_TABLES.items()]
     return out

@@ -5,10 +5,17 @@ path both misread shows up as a difference here.
 
 Only order-independent fields are produced: Count, Samples, the accepted-value Count, the sum (modulo 2^64 and
 unwrapped), Min / Max and the bucket counters.  Percentiles, stddev and sparse buckets depend on which block
-result is adopted first (Q9) and stay compared against the oracle through `tests.util.compare`.
+result is adopted first (Q9) and stay compared against the oracle through `tests.util.compare`.  Counters are
+kept as Python integers and compared wrapped to int64, as Go's `+= weight` leaves them.
+
+The result shaping (`ordered`: SortResults, OrderAsc, Limit) is restated as the engine's documented rule, see
+there.  StrReplace rewrites every decoded string of its column before filters and keys.
 
 `rows` is the list of `Spec.add_rows` calls as `(cols, block_rows, threshold)` and `valid` the parallel list of
 their validity masks ({name: bool array}; an absent name is fully valid)."""
+import math
+import re
+
 import numpy as np
 
 from tests.util import INT, SET, STR
@@ -231,12 +238,17 @@ def run(spec, rows, valid, q):
         lo, hi = infos[a]
         return Multi(lo, hi, pct, q.hist_bucket) if q.loghist else Basic(lo, hi, pct, q.hist_bucket)
 
+    # StrReplace (column_store_io.go:529-547 rewrites the block's string table): Go's $1 is Python's \g<1>
+    repl = {c: (re.compile(p), re.sub(r"\$(\d+)", r"\\g<\1>", r)) for c, (p, r) in q.str_replace.items()}
     for n, cells, info in blocks(spec, rows, valid):
         if not should_load(q, info):
             out.SkippedBlocks += 1
             continue
         # per column: values as Python objects, populated flags
         cv = {k: (v.tolist(), p.tolist()) for k, (v, p) in cells.items()}
+        for c, (pat, r) in repl.items():
+            if c in cv:  # a string rewritten to "" renders, and so groups, like a missing value
+                cv[c] = ([pat.sub(r, x) for x in cv[c][0]], cv[c][1])
         empty = ([0] * n, [False] * n)
         weight = 1  # declared per block, carried over rows without the weight column (Q13)
         for i in range(n):
@@ -326,63 +338,96 @@ def hist_fields(h):
     return h.Count, h.ExactSum, h.Min, h.Max, list(h.Values)
 
 
+def mean_value(g, a):
+    """The mean SortResults orders by, as the engine documents it: float(int64 Sum) / float(int64 hist Count), each
+    operand converted on its own as `(double)sum / (double)hc` does (not Python's correctly rounded int / int, which
+    differs above 2^53); -inf when the group has no histogram for `a` or its Count is 0."""
+    h = g.Hists.get(a)
+    hc = i64(h.Count) if h is not None else 0
+    return -math.inf if hc == 0 else float(i64(h.Sum)) / float(hc)
+
+
+def ordered(groups, q):
+    """SortResults + OrderAsc (aggregate.go:497-525) over {GroupByKey: Group}: the keys by Count (int64) or by
+    mean_value of aggregation q.order_by, descending, ties by GroupByKey ascending (Python str order, which is
+    UTF-8 byte order); OrderAsc reverses the whole list.  None for OrderBy "": any order is right.
+    The reference's own order is a float running mean under Go's unstable sort, so its ties fall either way
+    (aggregate.go:43-54,497-525; Q18/Q20): this restates the rule the engine and the oracle implement."""
+    if not q.order_by:
+        return None
+    if q.order_by == "$COUNT":
+        val = {k: i64(g.Count) for k, g in groups.items()}
+    else:
+        val = {k: mean_value(g, q.order_by) for k, g in groups.items()}
+    keys = sorted(sorted(groups), key=lambda k: val[k], reverse=True)  # (stable: ties keep key order)
+    return keys[::-1] if q.order_asc else keys
+
+
 def wrapped(r):
     """True when some group's sum left int64 (its mean is then a documented divergence, DESIGN.md §7)."""
     groups = list(r.Results.values()) + [r.Cumulative] + [g for m in r.TimeResults.values() for g in m.values()]
     return any(h.Sum != i64(h.Sum) for g in groups for h in g.Hists.values())
 
 
-def check(ref, got, q, hists_of=lambda g: g.Hists, where=""):
-    """got (oracle, pyoracle or engine result) against ref on every field rowref produces."""
+def check(ref, got, q, hists_of=lambda g: g.Hists, where="", order=True):
+    """got (oracle, pyoracle or engine result) against ref on every field rowref produces.  The engine (a result
+    with NumGroups) keeps the first `limit` groups of the sorted list; the oracle and pyoracle keep every group.
+    order=False compares the groups but not their order (the oracle's mean order is its float running mean)."""
     hist_mode = q.op == "hist" or q.loghist
 
     def grp(rg, gg, w):
-        assert (gg.Count, gg.Samples) == (rg.Count, rg.Samples), (w, "Count/Samples", (gg.Count, gg.Samples),
-                                                                  (rg.Count, rg.Samples))
+        assert (i64(gg.Count), gg.Samples) == (i64(rg.Count), rg.Samples), (w, "Count/Samples", (gg.Count, gg.Samples),
+                                                                            (rg.Count, rg.Samples))
         gh = hists_of(gg)
         for ai, a in enumerate(q.aggs if not (q.time_col and w[1] == "Results") else []):
             rh = rg.Hists.get(a)
             h = gh.get(a, gh.get(ai)) if isinstance(gh, dict) else None
-            if rh is None or rh.Count == 0:
-                assert h is None or hist_fields(h)[0] == 0, (w, a, "unexpected hist")
+            if rh is None or i64(rh.Count) == 0:
+                assert h is None or i64(hist_fields(h)[0]) == 0, (w, a, "unexpected hist")
                 continue
             assert h is not None, (w, a, "missing hist")
             c, s, mn, mx, vals = hist_fields(h)
             rc, rs, rmn, rmx, rvals = hist_fields(rh)
-            assert c == rc, (w, a, "hist Count", c, rc)
+            assert i64(c) == i64(rc), (w, a, "hist Count", c, rc)
             assert s == rs, (w, a, "sum mod 2^64", s, rs)
             if hist_mode:
                 assert (mn, mx) == (rmn, rmx), (w, a, "Min/Max", (mn, mx), (rmn, rmx))
             if q.op == "hist":
-                assert list(vals) == list(rvals), (w, a, "bucket counters",
-                                                   [(k, x, y) for k, (x, y) in enumerate(zip(vals, rvals)) if x != y][:8])
+                vals, rvals = [i64(int(x)) for x in vals], [i64(x) for x in rvals]
+                assert vals == rvals, (w, a, "bucket counters",
+                                       [(k, x, y) for k, (x, y) in enumerate(zip(vals, rvals)) if x != y][:8])
+
+    def keys_in_order(got_keys, groups, w):
+        """got_keys (a result list's keys in its order) against `groups` shaped by ordered() and the limit."""
+        assert len(got_keys) == len(set(got_keys)), (w, "groups sharing a key",
+                                                     sorted(k for k in set(got_keys) if got_keys.count(k) > 1)[:8])
+        want = ordered(groups, q)
+        cut = q.limit if q.limit and hasattr(got, "NumGroups") and w[-1] == "Sorted" else None
+        if want is None:  # OrderBy "": any `limit` of the groups, each exact
+            assert len(got_keys) == len(list(groups)[:cut]), (w, "groups", len(got_keys), len(groups))
+            assert set(got_keys) <= set(groups), (w, "group keys", sorted(set(got_keys) - set(groups))[:8])
+            return
+        want = want[:cut]
+        if order and hasattr(got, "Sorted"):  # (pyoracle's Results have no order)
+            i = next((i for i, (x, y) in enumerate(zip(got_keys, want)) if x != y), min(len(got_keys), len(want)))
+            assert got_keys == want, (w, "order", len(got_keys), len(want), "first difference at", i,
+                                      got_keys[i:i + 4], want[i:i + 4])
+        else:
+            assert set(got_keys) == set(want), (w, "group keys", sorted(set(got_keys) ^ set(want))[:8])
 
     assert got.MatchedCount == ref.MatchedCount, (where, "MatchedCount", got.MatchedCount, ref.MatchedCount)
     # Results is a dict keyed by the rendered key: two groups with one key would hide each other there, so the
-    # group counts are checked on the lists the dicts were built from
+    # group counts are checked on the lists the dicts were built from.  NumGroups counts every group, limit or not
     if hasattr(got, "NumGroups"):
         assert got.NumGroups == len(ref.Results), (where, "NumGroups", got.NumGroups, len(ref.Results))
     keys = [r.GroupByKey for r in getattr(got, "Sorted", None) or got.Results.values()]
-    assert len(keys) == len(set(keys)), (where, "groups sharing a key", sorted(k for k in set(keys)
-                                                                                if keys.count(k) > 1)[:8])
-    if q.limit:  # the first `limit` groups by Count descending; the tables keep the cut tie-free
-        order = sorted(ref.Results, key=lambda k: (-ref.Results[k].Count, k))
-        want = order[:q.limit]
-        if len(order) > q.limit:
-            assert ref.Results[order[q.limit - 1]].Count != ref.Results[order[q.limit]].Count, (where, "tie at the cut")
-        if hasattr(got, "NumGroups"):  # the engine materialises exactly the first `limit` groups
-            assert len(keys) == len(want), (where, "groups under limit", len(keys), len(want))
-        if hasattr(got, "Sorted"):
-            assert keys[:q.limit] == want, (where, "top groups", keys[:8], want[:8])
-        else:
-            assert set(want) <= set(keys), (where, "top groups")
-    else:
-        assert set(got.Results) == set(ref.Results), (where, "group keys",
-                                                      sorted(set(got.Results) ^ set(ref.Results))[:8])
+    keys_in_order(keys, ref.Results, (where, "Sorted"))
+    assert set(got.Results) == set(keys), (where, "Results against Sorted")
     for k in got.Results:
         grp(ref.Results[k], got.Results[k], (where, "Results", k))
     if q.time_col:
-        assert (got.Cumulative.Count, got.Cumulative.Samples) == (ref.Cumulative.Count, ref.Cumulative.Samples)
+        assert ((i64(got.Cumulative.Count), got.Cumulative.Samples) ==
+                (i64(ref.Cumulative.Count), ref.Cumulative.Samples)), (where, "Cumulative")
     else:
         grp(ref.Cumulative, got.Cumulative, (where, "Cumulative"))
     assert set(got.TimeResults) == set(ref.TimeResults), (where, "time buckets",
@@ -390,6 +435,8 @@ def check(ref, got, q, hists_of=lambda g: g.Hists, where=""):
     for tb, m in ref.TimeResults.items():
         n = getattr(got, "TimeNumGroups", {}).get(tb, len(got.TimeResults[tb]))
         assert n == len(m), (where, "time groups", tb, "groups sharing a key")
+        if hasattr(got, "TimeNumGroups"):  # the engine's slices are dicts built from its sorted lists
+            keys_in_order(list(got.TimeResults[tb]), m, (where, "TimeResults", tb))
         assert set(got.TimeResults[tb]) == set(m), (where, "time groups", tb)
         for k, rg in m.items():
             grp(rg, got.TimeResults[tb][k], (where, "TimeResults", tb, k))

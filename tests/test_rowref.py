@@ -33,8 +33,9 @@ def test_oracle_matches_rowref(name):
             o = run_oracle(spec, q)
             assert o.SkippedBlocks == ref.SkippedBlocks, (name, i, "skipped blocks")
             assert o.BrokenBlocks == 0
-            rowref.check(ref, o, q, where=(name, i, "oracle"))
-        if _nrows(rows) <= SMALL:
+            # the oracle orders by its float running mean (DESIGN.md §7): the order is compared for Count only
+            rowref.check(ref, o, q, where=(name, i, "oracle"), order=q.order_by == "$COUNT")
+        if _nrows(rows) <= SMALL and getattr(q, "pyoracle", True):
             rowref.check(ref, _Py(spec, q), q, where=(name, i, "pyoracle"))
 
 
