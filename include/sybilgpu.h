@@ -151,8 +151,10 @@ typedef struct sg_query_desc {
  *
  * Set columns (col_type SG_COL_SET, unpackSetCol column_store_io.go:611-688) come in the bucket form only:
  * Bins[i].Value = local string id of a tag, Bins[i].Records = the rows whose set holds it (a row may be listed
- * in several bins, never twice in one); at most SG_BLOCK_ROWS (bin,row) pairs per block in this build
- * (more: SG_ERR_UNSUPPORTED).  The host turns the non-bucketed file form (Values [][]int32, written for more
+ * in several bins, never twice in one).  A bin lists at most NumRecords rows (a longer one, or a row >= NumRecords,
+ * makes the block broken for queries that read the column, as the reference's "BLOCK SIZE CHANGED" does), and the
+ * block's arrays must fit the 64 MiB staging buffer (SG_ERR_INVALID otherwise); a column may list any number of
+ * (bin,row) pairs within those bounds.  The host turns the non-bucketed file form (Values [][]int32, written for more
  * than 5,000 distinct tags, column_store_io.go:183-192) into bins and passes len(Values) as `nvalues`: the
  * reference marks every row below it as populated, even with an empty set (column_store_io.go:672-682).
  *

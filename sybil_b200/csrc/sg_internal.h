@@ -27,6 +27,10 @@ enum : uint32_t {
   COL_SET = 1024u,        // set column (SavedSetColumn): bucket form, a row may sit in several bins; vmin holds the
                           // number of leading rows that are populated whatever the bins say (len(Values) of the
                           // non-bucketed file form, column_store_io.go:672-682)
+  COL_SEGS = 2048u,       // set column listing more than SG_BLOCK_ROWS (tag,row) pairs: this DevCol is its first segment,
+                          // vmax holds (number of further segments << 32) | index of the first of them in
+                          // LaunchParams::segs.  Every segment is a self-contained bucket column of whole bins (at most
+                          // SG_BLOCK_ROWS entries); none carries COL_TMA, so all are read with plain loads
 };
 // log2(4-byte-id or 8-byte-value width / stored width): the row pitch of the arena view a column's tiles are
 // fetched through is 128 >> shift bytes, so a warp tile always holds 1024 ids / 512 values
@@ -170,6 +174,7 @@ struct LaunchParams {
   const Plan* plan;
   const DevBlock* blocks;
   const DevCol* cols;         // [nblocks_table][ncolslots]
+  const DevCol* segs;         // continuation segments of COL_SEGS set columns (table-wide)
   const uint4* items;         // work items {block, mask, NumRecords, -}; mask bits 0..15 = aggregations this
                               // item computes, bit 31 = the item owns the block's Count / MatchedCount
   uint32_t nlist;

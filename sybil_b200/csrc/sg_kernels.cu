@@ -1643,15 +1643,26 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
         // sticky bits instead of a pass count — a row may be listed in several bins.  The planner keeps such a query
         // in count mode (fail_mode == 0).
         if (c.enc == SG_ENC_BUCKET) {
-          uint32_t* pay = c.nbins <= SMEM_BINS ? cx.binpay_s : gbinpay;
-          for (uint32_t b = cx.tid; b < c.nbins; b += THREADS)
-            pay[b] = F.set_pbit | (str_gid(c, c.bin_values[b]) == F.str_gid ? F.set_tbit : 0u);
-          __syncthreads();
-          scan_bucket<SlotT>(
-              cx, c, nrec, [&](uint32_t bin) { return (SlotT)pay[bin]; },
-              [&](uint32_t row, SlotT cur) {
-                if (cur) slot_or(slot, slot_s, row, (uint32_t)cur);
-              });
+          // A column with more than SG_BLOCK_ROWS pairs comes in segments of whole bins (COL_SEGS), each walked like
+          // a column of its own; the bits are ORed, so the order does not matter.  Under IN only the literal's bins
+          // set bits: a segment without one is not read at all (its rows were range-checked at staging).
+          const uint32_t nseg = (c.flags & COL_SEGS) ? 1u + (uint32_t)((unsigned long long)c.vmax >> 32) : 1u;
+          for (uint32_t s = 0; s < nseg; s++) {
+            const DevCol sc = s ? lp.segs[(uint32_t)c.vmax + s - 1u] : c;
+            uint32_t* pay = sc.nbins <= SMEM_BINS ? cx.binpay_s : gbinpay;
+            uint32_t any = 0;
+            for (uint32_t b = cx.tid; b < sc.nbins; b += THREADS) {
+              const uint32_t p = F.set_pbit | (str_gid(sc, sc.bin_values[b]) == F.str_gid ? F.set_tbit : 0u);
+              pay[b] = p;
+              any |= p;
+            }
+            if (!__syncthreads_or(any) && nseg > 1u) continue;
+            scan_bucket<SlotT>(
+                cx, sc, nrec, [&](uint32_t bin) { return (SlotT)pay[bin]; },
+                [&](uint32_t row, SlotT cur) {
+                  if (cur) slot_or(slot, slot_s, row, (uint32_t)cur);
+                });
+          }
         }
         // rows the non-bucketed file form listed (even with an empty set) are populated (a column of nothing but
         // empty sets is staged as ABSENT + COL_SET)

@@ -333,6 +333,7 @@ struct sg_table {
   std::vector<int32_t> types;
   std::vector<HostBlock> blocks;
   std::vector<DevCol> cols;  // [nblocks][ncols] host mirror (device pointers inside)
+  std::vector<DevCol> segs;  // continuation segments of COL_SEGS set columns (sg_internal.h), host mirror
   std::vector<StrDict> sdict;
   std::vector<IntDict> idict;
   // entries each dictionary held after its last sg_table_dict_seed_* call (-1: never seeded).  A dictionary that
@@ -390,6 +391,8 @@ struct sg_table {
   DevBlock* d_blocks = nullptr;
   DevCol* d_cols = nullptr;
   size_t d_blocks_cap = 0;
+  DevCol* d_segs = nullptr;
+  size_t d_segs_cap = 0;
   bool dirty = true;
   uint64_t version = 1;  // bumped whenever blocks or dictionaries change: a query's plan is reused while it stands
   // Small arrays of consecutive blocks (bin values, offsets, remap tables: a few KB per block) sit back to back both in
@@ -638,6 +641,7 @@ void sg_table_free(sg_table* t) {
   }
   if (t->d_blocks) cudaFree(t->d_blocks);
   if (t->d_cols) cudaFree(t->d_cols);
+  if (t->d_segs) cudaFree(t->d_segs);
   for (auto& vh : t->vhash) {
     if (vh.d_keys) cudaFree(vh.d_keys);
     if (vh.d_ids) cudaFree(vh.d_ids);
@@ -661,6 +665,49 @@ struct Premap {
     return host && c >= host && c + n <= host + bytes && ((size_t)(c - host) % 128) == 0;
   }
 };
+
+// One segment of a set column cut at bin boundaries: its first bin, its bin offsets rebased to its own ids, and
+// where its two arrays sit in the block's slab.
+struct SetSeg {
+  uint32_t b0 = 0;
+  std::vector<uint32_t> bo;
+  size_t off_bo = 0, off_data = 0;
+};
+
+// A set column listing more than SG_BLOCK_ROWS (tag,row) pairs is cut greedily into segments of whole bins, each of
+// at most SG_BLOCK_ROWS entries.  A bin's first id is absolute even with delta-encoded ids, so every segment is a
+// bucket column of its own.  `offs` are the offsets of the column's non-empty bins into record_ids (nbins + 1).
+// Returns false when the block is broken for this column: some row >= NumRecords, or a bin longer than
+// SG_BLOCK_ROWS (never two entries for one row in a bin, so it holds such a row).  The rows are checked here and
+// not only by the scan: an IN filter does not read the segments that lack its tag.
+static bool cut_set_segments(const sg_column_desc& cd, size_t id_size, uint32_t nrec, const std::vector<uint32_t>& offs,
+                             std::vector<SetSeg>& segs) {
+  auto rows_ok = [&](auto ids) {
+    for (size_t b = 0; b + 1 < offs.size(); b++) {
+      uint64_t row = 0;
+      for (uint32_t j = offs[b]; j < offs[b + 1]; j++) {
+        row = (cd.delta_ids && j > offs[b]) ? row + ids[j] : (uint64_t)ids[j];
+        if (row >= nrec) return false;
+      }
+    }
+    return true;
+  };
+  segs.clear();  // (left empty when the block is broken)
+  for (size_t b = 0; b + 1 < offs.size(); b++)
+    if (offs[b + 1] - offs[b] > SG_BLOCK_ROWS) return false;
+  if (!(id_size == 2 ? rows_ok((const uint16_t*)cd.record_ids) : rows_ok((const uint32_t*)cd.record_ids))) return false;
+  for (size_t b = 0; b + 1 < offs.size(); b++) {
+    if (segs.empty() || offs[b + 1] - offs[segs.back().b0] > SG_BLOCK_ROWS) {
+      segs.emplace_back();
+      segs.back().b0 = (uint32_t)b;
+    }
+  }
+  for (size_t s = 0; s < segs.size(); s++) {
+    const uint32_t b0 = segs[s].b0, b1 = s + 1 < segs.size() ? segs[s + 1].b0 : (uint32_t)offs.size() - 1u;
+    for (uint32_t b = b0; b <= b1; b++) segs[s].bo.push_back(offs[b] - offs[b0]);
+  }
+  return true;
+}
 }  // namespace
 
 static int add_block_impl(sg_table* t, const sg_block_desc* b, const Premap& pm) {
@@ -686,6 +733,7 @@ static int add_block_impl(sg_table* t, const sg_block_desc* b, const Premap& pm)
     size_t off_bv = 0, off_bo = 0, off_data = 0, off_remap = 0;
     bool has_bv = false, has_bo = false, has_data = false, has_remap = false;
     char* premapped = nullptr;  // the data array already sits in the arena (mirrored span)
+    std::vector<SetSeg> segs;   // a set column cut into segments (COL_SEGS)
   };
   std::vector<Tmp> tmp((size_t)b->ncols);
   SlabWriter sw;
@@ -801,11 +849,7 @@ static int add_block_impl(sg_table* t, const sg_block_desc* b, const Premap& pm)
         c->set_err("add_block: bin_offsets do not span record_ids");
         return SG_ERR_INVALID;
       }
-      if (cd.nrecord_ids > SG_BLOCK_ROWS) {
-        if (is_set) {
-          c->set_err("add_block: set column with more than 65,536 (tag,row) pairs in one block (not in this build)");
-          return SG_ERR_UNSUPPORTED;
-        }
+      if (cd.nrecord_ids > SG_BLOCK_ROWS && !is_set) {
         // more (bin,row) pairs than a block has rows: some row would be listed twice
         c->set_err("add_block: more record ids than rows in a block");
         return SG_ERR_INVALID;
@@ -861,15 +905,38 @@ static int add_block_impl(sg_table* t, const sg_block_desc* b, const Premap& pm)
         dc.vmax = mx;
         dc.flags |= COL_STATS;
       }
-      tm.off_bv = sw.add(tm.bin_values.data(), tm.bin_values.size() * 8);
-      tm.off_bo = sw.add(tm.bin_offsets.data(), tm.bin_offsets.size() * 4);
-      if (pm.has(cd.record_ids, (size_t)cd.nrecord_ids * id_size))
-        tm.premapped = pm.dev + ((const char*)cd.record_ids - pm.host);
-      else
-        tm.off_data = sw.add(cd.record_ids, (size_t)cd.nrecord_ids * id_size, c->is_pinned(cd.record_ids, (size_t)cd.nrecord_ids * id_size));
-      tm.has_bv = tm.has_bo = tm.has_data = true;
-      enc_bytes += (int64_t)(tm.bin_values.size() * 8 + tm.bin_offsets.size() * 4 + (size_t)cd.nrecord_ids * id_size);
-      if (cd.nrecord_ids == nrec && !is_set) stats_slots.push_back((uint32_t)cd.col_slot);  // candidate for COL_FULL
+      if (cd.nrecord_ids > SG_BLOCK_ROWS) {  // (a set column: int / str columns were refused above)
+        if (!cut_set_segments(cd, id_size, nrec, tm.bin_offsets, tm.segs)) {
+          // a row >= NumRecords: "BLOCK SIZE CHANGED DURING QUERY" (column_store_io.go:654-656), nothing to stage
+          dc.enc = SG_ENC_ABSENT;
+          dc.flags |= COL_BROKEN;
+          continue;
+        }
+        dc.flags |= COL_SEGS;
+        tm.off_bv = sw.add(tm.bin_values.data(), tm.bin_values.size() * 8);
+        // every segment's ids are a part of their own (128-byte aligned, as the tile loads assume): never a pointer
+        // into the middle of the caller's array, premapped or not
+        const char* ids = (const char*)cd.record_ids;
+        for (size_t s = 0; s < tm.segs.size(); s++) {
+          auto& sg = tm.segs[s];
+          const size_t e0 = tm.bin_offsets[sg.b0], n = sg.bo.back();
+          sg.off_bo = sw.add(sg.bo.data(), sg.bo.size() * 4);
+          sg.off_data = sw.add(ids + e0 * id_size, n * id_size, c->is_pinned(ids + e0 * id_size, n * id_size));
+          enc_bytes += (int64_t)(sg.bo.size() * 4);
+        }
+        tm.has_bv = true;
+        enc_bytes += (int64_t)(tm.bin_values.size() * 8 + (size_t)cd.nrecord_ids * id_size);
+      } else {
+        tm.off_bv = sw.add(tm.bin_values.data(), tm.bin_values.size() * 8);
+        tm.off_bo = sw.add(tm.bin_offsets.data(), tm.bin_offsets.size() * 4);
+        if (pm.has(cd.record_ids, (size_t)cd.nrecord_ids * id_size))
+          tm.premapped = pm.dev + ((const char*)cd.record_ids - pm.host);
+        else
+          tm.off_data = sw.add(cd.record_ids, (size_t)cd.nrecord_ids * id_size, c->is_pinned(cd.record_ids, (size_t)cd.nrecord_ids * id_size));
+        tm.has_bv = tm.has_bo = tm.has_data = true;
+        enc_bytes += (int64_t)(tm.bin_values.size() * 8 + tm.bin_offsets.size() * 4 + (size_t)cd.nrecord_ids * id_size);
+        if (cd.nrecord_ids == nrec && !is_set) stats_slots.push_back((uint32_t)cd.col_slot);  // candidate for COL_FULL
+      }
     } else if (cd.encoding == SG_ENC_VALUES) {
       dc.nitems = cd.nvalues;
       if (cd.nvalues > nrec) {
@@ -996,6 +1063,27 @@ static int add_block_impl(sg_table* t, const sg_block_desc* b, const Premap& pm)
       }
     }
     if (tm.has_remap) dc.remap = (const int32_t*)(dev + tm.off_remap);
+    if (!tm.segs.empty()) {
+      // the slot's DevCol is the first segment, the others follow in the table-wide segment array
+      const uint64_t first = t->segs.size();
+      for (size_t s = 0; s < tm.segs.size(); s++) {
+        const SetSeg& sg = tm.segs[s];
+        DevCol sc = dc;
+        sc.flags &= ~COL_SEGS;
+        sc.nbins = (uint32_t)sg.bo.size() - 1u;
+        sc.nitems = sg.bo.back();
+        sc.bin_values = (const int64_t*)(dev + tm.off_bv) + sg.b0;
+        sc.bin_offsets = (const uint32_t*)(dev + sg.off_bo);
+        sc.data = dev + sg.off_data;
+        if (s == 0) {
+          sc.flags |= COL_SEGS;
+          sc.vmax = (int64_t)(((uint64_t)(tm.segs.size() - 1) << 32) | first);
+          dc = sc;
+        } else {
+          t->segs.push_back(sc);
+        }
+      }
+    }
   }
   HostBlock hb;
   hb.block_index = b->block_index;
@@ -1089,6 +1177,7 @@ int sg_table_clear(sg_table* t) {
   CUDA_TRY(t->ctx, cudaStreamSynchronize(t->ctx->stream));
   t->blocks.clear();
   t->cols.clear();
+  t->segs.clear();
   t->pending_stats.clear();
   for (auto& vh : t->vhash) vh.blocks_done = 0;
   t->chunk_idx = 0;
@@ -1408,6 +1497,17 @@ int upload_table(sg_table* t) {
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));  // (H2D on the stream the kernels run on: see remap_to_union)
     CUDA_TRY(c, cudaMemcpyAsync(t->d_cols, t->cols.data(), nb * (size_t)t->ncols * sizeof(DevCol), cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));  // (H2D on the stream the kernels run on: see remap_to_union)
+  }
+  if (!t->segs.empty()) {
+    if (t->segs.size() > t->d_segs_cap) {
+      if (t->d_segs) cudaFree(t->d_segs);
+      t->d_segs = nullptr;
+      const size_t cap = std::max<size_t>(t->segs.size() * 2, 256);
+      CUDA_TRY(c, cudaMalloc(&t->d_segs, cap * sizeof(DevCol)));
+      t->d_segs_cap = cap;
+    }
+    CUDA_TRY(c, cudaMemcpyAsync(t->d_segs, t->segs.data(), t->segs.size() * sizeof(DevCol), cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(c, cudaStreamSynchronize(c->stream));
   }
   if (!t->pending_stats.empty()) {
     // exact extents of the newly staged value-array int columns (one more read of those
@@ -2280,6 +2380,7 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list) {
   lp.plan = q->d_plan;
   lp.blocks = t->d_blocks;
   lp.cols = t->d_cols;
+  lp.segs = t->d_segs;
   lp.items = reinterpret_cast<const uint4*>(q->d_block_list);
   lp.nlist = (uint32_t)items.size();
   lp.slot_bytes = q->slot_bytes;
@@ -2354,6 +2455,16 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list) {
             " hashg=%d gbits=%u fbits=%d tbit=%d count_bins=%u",
             q->variant->name, q->slot_bytes, P.acc_repl, lp.fold_every, P.fail_mode, P.hist_rows, P.lslots, P.nslots,
             q->hashed ? 1 : 0, q->hashg ? 1 : 0, P.gbits, __builtin_popcount(P.filt_mask), P.time_ok ? 1 : 0, count_bins);
+    for (int i = 0; i < P.nfilters; i++) {  // per set filter: the most segments its column has in a listed block
+      if (P.filters[i].op != SG_OP_IN && P.filters[i].op != SG_OP_NIN) continue;
+      uint32_t segs = 0;
+      for (uint32_t b : list) {
+        const DevCol& dc = t->cols[(size_t)b * (size_t)t->ncols + (size_t)P.filters[i].col];
+        if (dc.enc == SG_ENC_BUCKET)
+          segs = std::max(segs, (dc.flags & COL_SEGS) ? 1u + (uint32_t)((uint64_t)dc.vmax >> 32) : 1u);
+      }
+      fprintf(stderr, " set_segs=%u", segs);
+    }
     for (int a = 0; a < P.naggs; a++) {
       // the same expressions as scan_kernel's fast range, `hist32` and `nocarry` (R = acc_repl there)
       const KAgg& ka = P.aggs[a];
