@@ -31,6 +31,10 @@ enum : uint32_t {
                           // vmax holds (number of further segments << 32) | index of the first of them in
                           // LaunchParams::segs.  Every segment is a self-contained bucket column of whole bins (at most
                           // SG_BLOCK_ROWS entries); none carries COL_TMA, so all are read with plain loads
+  COL_CODES = 4096u,      // bucket int / str column of at most 255 bins whose rows the staging statistics kernel checked
+                          // (each listed once, all < NumRecords): `codes` holds every row's bin index as one byte in row
+                          // order, 0xFF for a row the column does not list, padded to 16 bytes.  The scan reads the
+                          // codes instead of walking the ids (no COL_TMA: the union below no longer locates the ids)
 };
 // log2(4-byte-id or 8-byte-value width / stored width): the row pitch of the arena view a column's tiles are
 // fetched through is 128 >> shift bytes, so a warp tile always holds 1024 ids / 512 values
@@ -55,8 +59,13 @@ struct DevCol {
   // exact extents of the decoded values (int columns), computed by the engine when the block is
   // staged (bucket columns: on the host from the bin values; value arrays: stats kernel)
   int64_t vmin, vmax;
-  // `data` as a coordinate of the arena chunk's tensor map ({128 B, rows}): row = byte offset / 128
-  uint32_t data_chunk, data_row;
+  union {
+    // COL_TMA: `data` as a coordinate of the arena chunk's tensor map ({128 B, rows}): row = byte offset / 128
+    struct {
+      uint32_t data_chunk, data_row;
+    };
+    const uint8_t* codes;  // COL_CODES: per-row bin indices (see there)
+  };
 };
 static_assert(sizeof(DevCol) == 80, "DevCol layout");
 
@@ -223,9 +232,10 @@ __host__ __device__ static inline uint32_t vh_hash(long long v) {
 #define SG_DECLARE_VARIANT(ns)                                                                                          \
   namespace ns {                                                                                                        \
   int launch_scan(const LaunchParams& lp, int grid, void* stream);                                                      \
-  /* extents of value-array int columns: items[i] = index into cols[] (block * ncolslots + slot) */                    \
-  int launch_stats(DevCol* cols, const DevBlock* blocks, const uint32_t* items, uint32_t nitems, uint32_t ncolslots,    \
-                   void* stream);                                                                                       \
+  /* extents of value-array int columns, COL_FULL and COL_CODES of bucket columns: items[i] = index into cols[]       \
+   * (block * ncolslots + slot), codes[i] = where item i's per-row codes go (0: none) */                               \
+  int launch_stats(DevCol* cols, const DevBlock* blocks, const uint32_t* items, const unsigned long long* codes,       \
+                   uint32_t nitems, uint32_t ncolslots, void* stream);                                                  \
   /* distinct values of value-array int columns: keys[cap] (pre-filled with INT64_MIN = empty) receives every          \
    * distinct decoded value of the listed (block, column) items; counters[0] += new keys, counters[1] = 1 if          \
    * INT64_MIN itself occurred, counters[2] = 1 if the set filled up (more than cap/2 keys) */                          \

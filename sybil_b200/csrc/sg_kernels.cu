@@ -56,6 +56,11 @@ constexpr int BE = 32;  // row ids per lane in a bucket tile  (tile = 1024 ids, 
 constexpr int VE = 16;  // int64 values per lane in a value tile (tile = 512 rows, 4 KB)
 constexpr int SE = 8;   // int32 string ids per lane (tile = 256 rows)
 constexpr uint32_t MAX_TILES = 128;
+// the code pass (COL_CODES columns): how a column's payload joins the row's slot word, and its payload table (one
+// entry per code; code 0xFF, an unlisted row, reads 0)
+enum : uint32_t { CODE_ADD = 0, CODE_OR = 1, CODE_TIME = 2 };
+constexpr uint32_t CODE_BINS = 256;
+constexpr uint32_t CODE_BATCH = SMEM_BINS / CODE_BINS;  // code columns whose loads are issued together (4)
 
 int scan_threads() { return THREADS; }
 
@@ -1545,49 +1550,63 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
     const DevCol* __restrict__ cols = lp.cols + (size_t)bid * ncolslots;
 
     // the block's TMA-fed passes in execution order (mirrors the pass sequence below): one thread
-    // per candidate looks its column up, warp 0 compacts after the barrier
+    // per candidate looks its column up, warp 0 compacts after the barrier.  ptmp[4 * i]: bit 0 TMA-fed,
+    // bit 1 read in the code pass (COL_CODES filter / group / time column), bits 2.. its CODE_* role
+    bool my_code = false;
     if ((uint32_t)cx.tid < ncand) {
       const uint32_t pc = pcand[cx.tid];
       const uint32_t kind = (pc >> 16) & 0xffu;
       const DevCol c = cols[pc & 0xffu];
       bool on = cx.tmaps != nullptr && (c.flags & COL_TMA) && cx.stages(col_shift(c.flags)) != 0u;
       bool bucket = c.enc == SG_ENC_BUCKET;
+      const bool coded = bucket && (c.flags & COL_CODES);
+      uint32_t role = CODE_ADD;
       if (kind == 0) {
         // (a bucket filter in fail mode walks only the tiles of its failing bins, with plain loads)
         on = on && ((bucket && !fail_mode) || (c.enc == SG_ENC_VALUES && !(pc >> 24)));
+        my_code = coded && PP->filters[cx.tid].op < SG_OP_IN;
+        if (fail_mode) role = CODE_OR;
       } else if (kind == 1) {
         on = on && (bucket || (HASHG && c.enc == SG_ENC_VALUES && !(c.flags & COL_IS_STR)));
+        my_code = coded;
       } else {
         on = on && !(c.flags & COL_IS_STR) && (bucket || c.enc == SG_ENC_VALUES);
         if (kind == 3) on = on && ((aggmask >> ((pc >> 8) & 0xffu)) & 1u);
-        if (kind == 2 && on && (c.enc == SG_ENC_VALUES || (bucket && (c.flags & COL_FULL))) && (c.flags & COL_STATS)) {
+        bool cconst = false;
+        if (kind == 2 && (c.enc == SG_ENC_VALUES || (bucket && (c.flags & COL_FULL))) && (c.flags & COL_STATS) &&
+            !(c.flags & COL_IS_STR)) {
           // a fully populated time column whose extents fall into one time bucket is not read at all
           const uint32_t clo = time_code(c.vmin, PP->time_bucket, PP->time_first, PP->time_radix);
-          if (clo != 0u && clo == time_code(c.vmax, PP->time_bucket, PP->time_first, PP->time_radix)) on = false;
+          cconst = clo != 0u && clo == time_code(c.vmax, PP->time_bucket, PP->time_first, PP->time_radix);
         }
+        if (cconst) on = false;
+        my_code = kind == 2 && coded && !(c.flags & COL_IS_STR) && !cconst;
+        role = CODE_TIME;
       }
       uint32_t n = c.nitems;
       if (!bucket && n > nrec) n = nrec;
       colcache[cx.tid] = c;
-      ptmp[4 * cx.tid + 0] = on ? 1u : 0u;
+      ptmp[4 * cx.tid + 0] = (on ? 1u : 0u) | (my_code ? 2u | (role << 2) : 0u);
       ptmp[4 * cx.tid + 1] = c.data_chunk * 3u + col_shift(c.flags);  // which view of the chunk (see make_feed)
       ptmp[4 * cx.tid + 2] = c.data_row << col_shift(c.flags);
       ptmp[4 * cx.tid + 3] = bucket ? (n + (32 * BE - 1)) / (32 * BE) : (n + (32 * VE - 1)) / (32 * VE);
     }
-    // every row starts as: group slot 0, no filter passed
-    if (sizeof(SlotT) < 4) {
-      uint4* s4 = reinterpret_cast<uint4*>(slot);
-      const uint32_t n16 = (nrec * (uint32_t)sizeof(SlotT) + 15u) / 16u;
-      for (uint32_t i = cx.tid; i < n16; i += THREADS) s4[i] = make_uint4(0, 0, 0, 0);
-    } else {
-      for (uint32_t r = cx.tid; r < nrec; r += THREADS) slot[r] = 0;
+    const bool code_pass = __syncthreads_or(my_code) != 0;
+    // every row starts as: group slot 0, no filter passed (the code pass, when there is one, stores every row's word)
+    if (!code_pass) {
+      if (sizeof(SlotT) < 4) {
+        uint4* s4 = reinterpret_cast<uint4*>(slot);
+        const uint32_t n16 = (nrec * (uint32_t)sizeof(SlotT) + 15u) / 16u;
+        for (uint32_t i = cx.tid; i < n16; i += THREADS) s4[i] = make_uint4(0, 0, 0, 0);
+      } else {
+        for (uint32_t r = cx.tid; r < nrec; r += THREADS) slot[r] = 0;
+      }
     }
-    __syncthreads();
     if (cx.warp == 0) {
       uint32_t np = 0;
       for (uint32_t b0 = 0; b0 < ncand; b0 += 32) {
         const uint32_t i = b0 + cx.lane;
-        const bool on = i < ncand && ptmp[4 * i] != 0;
+        const bool on = i < ncand && (ptmp[4 * i] & 1u) != 0;
         const uint32_t m = __ballot_sync(FULL, on);
         if (on) {
           const uint32_t pos = np + __popc(m & ((1u << cx.lane) - 1u));
@@ -1620,9 +1639,120 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
       hist_tb = tb;
     }
     hist_blocks++;
+    auto rel_of = [&](uint32_t code) -> uint32_t {  // global time code (0 = off the axis) -> window-relative, 0 = bad
+      const uint32_t r = code - tcode0 + 1u;
+      return (code != 0u && r >= 1u && r <= twin) ? r : 0u;
+    };
+    // Count without touching a row: with no filter, no time column and ONE group column whose bins list every
+    // row of the block exactly once (COL_FULL), a group's Count in this block is the size of its bin
+    const bool count_in_group = ACC_SMEM && nfilters == 0 && time_col < 0 && ngroups == 1 &&
+                                colcache[0].enc == SG_ENC_BUCKET && (colcache[0].flags & COL_FULL) != 0u;
     phase(0);
     pass_mark(-1);
     int pass_no = 0;
+
+    // ---- code pass: every COL_CODES filter, group and time column of the block in ONE row-ordered loop -------
+    // A column's per-bin payload is what its own pass below would give the rows of that bin; each lane then reads
+    // 16 consecutive rows' codes of every such column (16 bytes each), looks the payloads up and stores the 16 slot
+    // words: the first writer of every row (the zeroing above is skipped), no head bits, no look-back, no atomics.
+    if (code_pass) {
+      uint32_t ncode = 0;
+      const SlotT fincS = (SlotT)finc;
+      for (uint32_t i = 0; i < ncand; i++) {
+        const uint32_t f = ptmp[4 * i];
+        if (!(f & 2u)) continue;
+        const DevCol& c = colcache[i];
+        const uint32_t kind = (pcand[i] >> 16) & 0xffu;
+        uint32_t* const pay = (ncode + 1u) * CODE_BINS <= SMEM_BINS ? cx.binpay_s + ncode * CODE_BINS : gbinpay + ncode * CODE_BINS;
+        for (uint32_t b = cx.tid; b < CODE_BINS; b += THREADS) {
+          uint32_t p = 0;
+          if (b < c.nbins) {
+            if (kind == 0) {
+              const KFilter& F = PP->filters[i];
+              StrPred sp;
+              sp.op = F.op;
+              sp.gid = F.str_gid;
+              sp.lut = F.lut;
+              sp.lut_bits = F.lut_bits;
+              const long long bv = c.bin_values[b];
+              const bool pass = F.is_str ? sp(str_gid(c, bv)) : int_pred(F.op, bv, F.ival);
+              p = (pass != fail_mode) ? (uint32_t)fincS : 0u;  // count mode: finc = passes; fail mode: finc = fails
+            } else if (kind == 1) {
+              const KGroup& G = PP->groups[i - (uint32_t)nfilters];
+              const int32_t code = G.is_str ? str_gid(c, c.bin_values[b]) : c.remap[b];
+              p = code == G.alias ? 0u : ((uint32_t)code + 1u) * G.stride;
+              if (count_in_group)
+                sred_add(smem_u32(cx.acc + p * gstride + lane_off), c.bin_offsets[b + 1] - c.bin_offsets[b]);
+            } else {
+              const uint32_t rc = rel_of(time_code(c.bin_values[b], tbk, tfirst, tradix));
+              p = rc ? rc * tstride + time_ok : 0u;  // 0: counted into scalars[2] below
+            }
+          }
+          pay[b] = p;
+        }
+        if (cx.tid == 0) ptmp[4 * ncode + 1] = i | ((f >> 2) << 8);  // (ncode <= i: no flag word is overwritten)
+        ncode++;
+      }
+      __syncthreads();
+      unsigned long long ovf = 0;  // listed rows outside the time window
+      const uint32_t pay_s = smem_u32(cx.binpay_s);
+      for (uint32_t idx0 = (uint32_t)cx.tid * 16u; idx0 < nrec; idx0 += THREADS * 16u) {
+        uint32_t w[16];
+#pragma unroll
+        for (int k = 0; k < 16; k++) w[k] = 0u;
+        // columns in groups of CODE_BATCH: their loads are in flight together (the first group's tables are in
+        // shared memory, any further ones in gbinpay)
+        for (uint32_t j0 = 0; j0 < ncode; j0 += CODE_BATCH) {
+          uint4 q[CODE_BATCH];
+          uint32_t role[CODE_BATCH];
+#pragma unroll
+          for (uint32_t jj = 0; jj < CODE_BATCH; jj++) {
+            q[jj] = make_uint4(FULL, FULL, FULL, FULL);
+            role[jj] = CODE_ADD;
+            if (j0 + jj < ncode) {
+              const uint32_t e = ptmp[4 * (j0 + jj) + 1];
+              role[jj] = e >> 8;
+              q[jj] = __ldg(reinterpret_cast<const uint4*>(colcache[e & 0xffu].codes + idx0));
+            }
+          }
+#pragma unroll
+          for (uint32_t jj = 0; jj < CODE_BATCH; jj++) {
+            if (j0 + jj >= ncode) break;
+            const uint32_t cw[4] = {q[jj].x, q[jj].y, q[jj].z, q[jj].w};
+#pragma unroll
+            for (int k = 0; k < 16; k++) {
+              const uint32_t code = (cw[k >> 2] >> (8 * (k & 3))) & 0xffu;
+              uint32_t v;
+              if (j0 == 0)
+                asm("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(pay_s + (jj * CODE_BINS + code) * 4u));
+              else
+                v = gbinpay[(j0 + jj) * CODE_BINS + code];
+              w[k] = role[jj] == CODE_OR ? (w[k] | v) : (w[k] + v);
+              if (role[jj] == CODE_TIME && v == 0u && code != 0xffu) ovf++;
+            }
+          }
+        }
+        if (sizeof(SlotT) == 1) {
+          uint32_t p[4];
+#pragma unroll
+          for (int j = 0; j < 4; j++) p[j] = w[4 * j] | (w[4 * j + 1] << 8) | (w[4 * j + 2] << 16) | (w[4 * j + 3] << 24);
+          *reinterpret_cast<uint4*>(slot + idx0) = make_uint4(p[0], p[1], p[2], p[3]);
+        } else if (sizeof(SlotT) == 2) {
+          uint32_t p[8];
+#pragma unroll
+          for (int j = 0; j < 8; j++) p[j] = w[2 * j] | (w[2 * j + 1] << 16);
+          reinterpret_cast<uint4*>(slot + idx0)[0] = make_uint4(p[0], p[1], p[2], p[3]);
+          reinterpret_cast<uint4*>(slot + idx0)[1] = make_uint4(p[4], p[5], p[6], p[7]);
+        } else {
+#pragma unroll
+          for (int j = 0; j < 4; j++)
+            reinterpret_cast<uint4*>(slot + idx0)[j] = make_uint4(w[4 * j], w[4 * j + 1], w[4 * j + 2], w[4 * j + 3]);
+        }
+      }
+      if (ovf) gred_add(g_scalars + 2, ovf);
+      __syncthreads();
+      pass_mark(pass_no++);
+    }
 
     // ---- filters (aggregate.go:105-112; unpopulated -> false, Q1) -----------------
     // Count mode: a row collects finc per filter it passes (an unpopulated row passes none).  Fail mode
@@ -1630,6 +1760,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
     // a filter gets the sticky FAIL bit (finc) OR-ed in — a bucket column then only walks the tiles
     // that hold entries of its FAILING bins.
     for (int fi = 0; fi < nfilters; fi++) {
+      if (ptmp[4 * fi] & 2u) continue;  // read in the code pass
       const KFilter F = PP->filters[fi];
       const DevCol c = colcache[fi];
       const SlotT fincS = (SlotT)finc;
@@ -1772,15 +1903,14 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
 
     phase(1);
     // ---- group key (aggregate.go:125-143) as a dense mixed-radix index ---------------
-    // Count without touching a row: with no filter, no time column and ONE group column whose bins list every
-    // row of the block exactly once (COL_FULL), a group's Count in this block is the size of its bin
-    bool count_in_group = false;
+    // (the first pass to touch the slot words, when there is no filter and no code pass, stores instead of adding)
     for (int gi = 0; gi < ngroups; gi++) {
+      if (ptmp[4 * (nfilters + gi)] & 2u) continue;  // read in the code pass
       const KGroup G = PP->groups[gi];
       const DevCol c = colcache[nfilters + gi];
+      const bool first = nfilters == 0 && gi == 0 && !code_pass;
       if (c.enc == SG_ENC_BUCKET) {
         uint32_t* pay = c.nbins <= SMEM_BINS ? cx.binpay_s : gbinpay;
-        count_in_group = ACC_SMEM && nfilters == 0 && time_col < 0 && ngroups == 1 && (c.flags & COL_FULL) != 0u;
         for (uint32_t b = cx.tid; b < c.nbins; b += THREADS) {
           const int32_t code = G.is_str ? str_gid(c, c.bin_values[b]) : c.remap[b];
           pay[b] = code == G.alias ? 0u : ((uint32_t)code + 1u) * G.stride;
@@ -1788,7 +1918,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
             sred_add(smem_u32(cx.acc + pay[b] * gstride + lane_off), c.bin_offsets[b + 1] - c.bin_offsets[b]);
         }
         __syncthreads();
-        if (nfilters == 0 && gi == 0) {
+        if (first) {
           // first pass to touch the (zeroed) slot words: a plain store (measured on C2: 20% faster than the
           // reduction for this pass)
           scan_bucket<SlotT>(
@@ -1806,7 +1936,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
           const int32_t gid = str_gid(c, local);
           return gid == alias ? 0u : ((uint32_t)gid + 1u) * stride;
         };
-        if (nfilters == 0 && gi == 0) {
+        if (first) {
           // first pass to touch the zeroed slot words: a store, not a read-modify-write (with the slot words in
           // the global scratch the load was the top stall of the high-cardinality plan)
           scan_values_i32(cx, c, nrec, [&](uint32_t row, int32_t local) { slot[row] = (SlotT)word(local); });
@@ -1852,15 +1982,12 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
     // The slot word takes the code relative to the block's window (1..twin; see Plan).  A row outside
     // the planned axis — or outside the window, which the exact extents rule out — is counted in
     // scalars[2] and fails the query on the host.
-    if (time_col >= 0) {
+    const bool time_pass = time_col >= 0 && !(ptmp[4 * (nfilters + ngroups)] & 2u);  // (else read in the code pass)
+    if (time_pass) {
       const DevCol c = colcache[nfilters + ngroups];
       const SlotT tok = (SlotT)time_ok;
       const long long tb64 = tbk, tf = tfirst;
       const uint32_t tr = tradix, ts = tstride;
-      auto rel_of = [&](uint32_t code) -> uint32_t {  // global code (0 = off the axis) -> window-relative, 0 = bad
-        const uint32_t r = code - tcode0 + 1u;
-        return (code != 0u && r >= 1u && r <= twin) ? r : 0u;
-      };
       // every populated row of the block in ONE time bucket (exact extents): the column is not read
       const bool all_rows = c.enc == SG_ENC_VALUES || (c.enc == SG_ENC_BUCKET && (c.flags & COL_FULL));
       uint32_t cconst = 0;
@@ -1950,7 +2077,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
       }
     }
     __syncthreads();
-    if (time_col >= 0) pass_mark(pass_no++);
+    if (time_pass) pass_mark(pass_no++);
 
     // ---- hashed slot space (LaunchParams::hkeys): code -> index of an open-addressing table in global memory.
     // Only rows that passed every filter (and carry a time code in time mode) take a slot.  The reference keys a Go
@@ -2118,7 +2245,22 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
         agg_slow(&AS, e, v, 1);
       };
 
-      if (c.enc == SG_ENC_BUCKET) {
+      if (c.enc == SG_ENC_BUCKET && (c.flags & COL_CODES)) {
+        // per-row codes: the rows in order, each with its bin's value
+        const int64_t* __restrict__ bv = c.bin_values;
+        for (uint32_t idx0 = (uint32_t)cx.tid * 16u; idx0 < nrec; idx0 += THREADS * 16u) {
+          const uint4 q = __ldg(reinterpret_cast<const uint4*>(c.codes + idx0));
+          const uint32_t cw[4] = {q.x, q.y, q.z, q.w};
+          uint32_t sw[VE];
+          load_slots(slot, idx0, sw);
+#pragma unroll
+          for (int k = 0; k < 16; k++) {
+            const uint32_t code = (cw[k >> 2] >> (8 * (k & 3))) & 0xffu;
+            if (code != 0xffu) accept_one(sw[k], bv[code]);
+          }
+        }
+        __syncthreads();
+      } else if (c.enc == SG_ENC_BUCKET) {
         scan_bucket<long long>(
             cx, c, nrec, [&](uint32_t bin) { return (long long)c.bin_values[bin]; },
             [&](uint32_t row, long long curv) { accept_one((uint32_t)slot[row], curv); });
@@ -2460,13 +2602,18 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
 // staging-time statistics: exact min / max of the decoded values of value-array int
 // columns (one CTA per column of a block).  They let the scan kernel pick 32-bit
 // arithmetic and drop per-row range checks when a column provably needs neither.
+// Bucket columns get COL_FULL and, when the host reserved room for them, their per-row codes
+// (COL_CODES) from the same walk.
 // ---------------------------------------------------------------------------
+constexpr uint32_t STATS_DYN_SMEM = SG_BLOCK_ROWS;  // the per-row codes of one block, built in shared memory
 __global__ void __launch_bounds__(THREADS, 1) stats_kernel(DevCol* cols, const DevBlock* blocks,
-                                                           const uint32_t* items, uint32_t nitems,
-                                                           uint32_t ncolslots) {
+                                                           const uint32_t* items, const unsigned long long* codes,
+                                                           uint32_t nitems, uint32_t ncolslots) {
   __shared__ __align__(16) unsigned char smem_s[FIXED_SMEM];
   __shared__ long long red_min[NWARPS], red_max[NWARPS];
   __shared__ uint32_t rowbits[HEAD_WORDS];  // bucket columns: one bit per listed row
+  extern __shared__ uint4 codes_s4[];       // [STATS_DYN_SMEM / 16]
+  uint8_t* const codes_s = reinterpret_cast<uint8_t*>(codes_s4);
   Ctx cx;
   cx.tid = threadIdx.x;
   cx.lane = threadIdx.x & 31;
@@ -2501,23 +2648,47 @@ __global__ void __launch_bounds__(THREADS, 1) stats_kernel(DevCol* cols, const D
       // COL_FULL: the bins list every row of [0, NumRecords) exactly once — as many entries as rows,
       // every decoded id in range, no id twice.  Then no row is unpopulated for this column and a
       // filter may reason about the complement of a set of bins.
-      if (c.nitems != nrec) continue;
+      // COL_CODES (the host reserved `codes[it]`, nbins <= 255): the bin index of every row, 0xFF for an
+      // unlisted one.  Kept only when the walk found no row listed twice, no row >= NumRecords, no gap
+      // >= 65,536 and no bad bin index; otherwise the column stays with its ids alone.
+      uint8_t* const dst = reinterpret_cast<uint8_t*>(codes[it]);
+      if (c.nitems != nrec && !dst) continue;
       for (uint32_t i = cx.tid; i < HEAD_WORDS; i += THREADS) rowbits[i] = 0;
-      if (cx.tid == 0) cx.misc[1] = 0;
+      if (dst)
+        for (uint32_t i = cx.tid; i < SG_BLOCK_ROWS / 16; i += THREADS) codes_s4[i] = make_uint4(FULL, FULL, FULL, FULL);
+      if (cx.tid == 0) {
+        cx.misc[1] = 0;
+        cx.misc[2] = 0;  // a row listed twice
+      }
       __syncthreads();
       scan_bucket<uint32_t>(
-          cx, c, nrec, [&](uint32_t) { return 0u; },
-          [&](uint32_t row, uint32_t) { atomicOr(&rowbits[row >> 5], 1u << (row & 31)); });
+          cx, c, nrec, [&](uint32_t bin) { return bin; },
+          [&](uint32_t row, uint32_t bin) {
+            const uint32_t bit = 1u << (row & 31);
+            if (atomicOr(&rowbits[row >> 5], bit) & bit) cx.misc[2] = 1;
+            if (dst) codes_s[row] = (uint8_t)bin;
+          });
       uint32_t pc = 0;
       for (uint32_t i = cx.tid; i < HEAD_WORDS; i += THREADS) pc += (uint32_t)__popc(rowbits[i]);
 #pragma unroll
       for (int d = 16; d > 0; d >>= 1) pc += __shfl_xor_sync(FULL, pc, d);
       if (cx.lane == 0) red_min[cx.warp] = (long long)pc;
       __syncthreads();
+      const bool clean = cx.misc[1] == 0 && cx.misc[2] == 0;
+      if (dst && clean) {
+        uint4* const d4 = reinterpret_cast<uint4*>(dst);
+        for (uint32_t i = cx.tid; i < (nrec + 15u) / 16u; i += THREADS) d4[i] = codes_s4[i];
+      }
       if (cx.tid == 0) {
         long long tot = 0;
         for (int w = 0; w < NWARPS; w++) tot += red_min[w];
-        if (tot == (long long)nrec && cx.misc[1] == 0) cols[ci].flags = c.flags | COL_FULL;
+        uint32_t fl = c.flags;
+        if (c.nitems == nrec && tot == (long long)nrec && cx.misc[1] == 0) fl |= COL_FULL;
+        if (dst && clean) {
+          fl = (fl | COL_CODES) & ~COL_TMA;
+          cols[ci].codes = dst;
+        }
+        cols[ci].flags = fl;
       }
       __syncthreads();
       continue;
@@ -2640,14 +2811,16 @@ int launch_distinct(const DevCol* cols, const DevBlock* blocks, const uint32_t* 
   return (int)cudaGetLastError();
 }
 
-int launch_stats(DevCol* cols, const DevBlock* blocks, const uint32_t* items, uint32_t nitems, uint32_t ncolslots,
-                 void* stream) {
+int launch_stats(DevCol* cols, const DevBlock* blocks, const uint32_t* items, const unsigned long long* codes,
+                 uint32_t nitems, uint32_t ncolslots, void* stream) {
   if (nitems == 0) return 0;
   int dev = 0, sms = 148;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const uint32_t grid = nitems < (uint32_t)sms * 2 ? nitems : (uint32_t)sms * 2;
-  stats_kernel<<<grid, THREADS, 0, (cudaStream_t)stream>>>(cols, blocks, items, nitems, ncolslots);
+  const cudaError_t e = cudaFuncSetAttribute(stats_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)STATS_DYN_SMEM);
+  if (e != cudaSuccess) return (int)e;
+  stats_kernel<<<grid, THREADS, STATS_DYN_SMEM, (cudaStream_t)stream>>>(cols, blocks, items, codes, nitems, ncolslots);
   return (int)cudaGetLastError();
 }
 

@@ -366,6 +366,12 @@ struct sg_table {
   };
   std::vector<ValueHash> vhash;
   std::vector<uint32_t> pending_stats;  // value-array int columns whose extents are not computed yet
+  std::vector<unsigned long long> pending_codes;  // parallel to pending_stats: where the item's per-row codes go (0: none)
+  // The per-row codes of COL_CODES columns (sg_internal.h) are written on the device by the statistics kernel, so they
+  // get a bump allocator of their own: in the arena they would sit between the slabs of consecutive blocks and split
+  // the slabs' merged copies (and a merged copy over them would send their bytes over PCIe for nothing)
+  std::vector<std::pair<char*, size_t>> code_chunks;
+  size_t code_idx = 0, code_used = 0;
   // sort ranks of the dictionaries' rendered fields (ties of SortResults break by GroupByKey ascending):
   // rank[id] over the strings (resp. the decimal renderings of the int values) + '\t'; rebuilt when a
   // dictionary has grown.  splain[col]: no string of srank[col]'s dictionary holds a byte <= '\t' (the ranks
@@ -457,6 +463,30 @@ int arena_alloc(sg_table* t, size_t bytes, char** out) {
   }
   *out = t->chunks[t->chunk_idx].first + t->chunk_used;
   t->chunk_used += bytes;
+  return SG_OK;
+}
+
+constexpr size_t CODE_CHUNK = (size_t)64 << 20;
+int code_alloc(sg_table* t, size_t bytes, char** out) {
+  bytes = align_up(bytes, 128);
+  while (t->code_idx < t->code_chunks.size() && t->code_used + bytes > t->code_chunks[t->code_idx].second) {
+    t->code_idx++;
+    t->code_used = 0;
+  }
+  if (t->code_idx >= t->code_chunks.size()) {
+    char* p = nullptr;
+    cudaError_t e = cudaMalloc(&p, CODE_CHUNK);
+    if (e != cudaSuccess) {
+      t->ctx->set_err(std::string("cudaMalloc codes: ") + cudaGetErrorString(e));
+      return SG_ERR_NOMEM;
+    }
+    t->code_chunks.emplace_back(p, CODE_CHUNK);
+    t->code_idx = t->code_chunks.size() - 1;
+    t->code_used = 0;
+    t->device_bytes += (int64_t)CODE_CHUNK;
+  }
+  *out = t->code_chunks[t->code_idx].first + t->code_used;
+  t->code_used += bytes;
   return SG_OK;
 }
 
@@ -635,6 +665,7 @@ void sg_table_free(sg_table* t) {
   cudaSetDevice(t->ctx->device);
   cudaStreamSynchronize(t->ctx->copy_stream);
   for (auto& p : t->chunks) cudaFree(p.first);
+  for (auto& p : t->code_chunks) cudaFree(p.first);
   for (int i = 0; i < 2; i++) {
     if (t->stage[i].host) cudaFreeHost(t->stage[i].host);
     if (t->stage[i].done) cudaEventDestroy(t->stage[i].done);
@@ -739,6 +770,7 @@ static int add_block_impl(sg_table* t, const sg_block_desc* b, const Premap& pm)
   SlabWriter sw;
   int64_t enc_bytes = 0;
   std::vector<uint32_t> stats_slots;
+  std::vector<unsigned long long> stats_codes;  // parallel: where the column's per-row codes go (0: none)
 
   for (int ci = 0; ci < b->ncols; ci++) {
     const sg_column_desc& cd = b->cols[ci];
@@ -935,7 +967,18 @@ static int add_block_impl(sg_table* t, const sg_block_desc* b, const Premap& pm)
           tm.off_data = sw.add(cd.record_ids, (size_t)cd.nrecord_ids * id_size, c->is_pinned(cd.record_ids, (size_t)cd.nrecord_ids * id_size));
         tm.has_bv = tm.has_bo = tm.has_data = true;
         enc_bytes += (int64_t)(tm.bin_values.size() * 8 + tm.bin_offsets.size() * 4 + (size_t)cd.nrecord_ids * id_size);
-        if (cd.nrecord_ids == nrec && !is_set) stats_slots.push_back((uint32_t)cd.col_slot);  // candidate for COL_FULL
+        // candidate for COL_FULL, and for COL_CODES: room for one byte per row, which the statistics kernel fills
+        // when the walk finds every listed row once and in range (SG_NO_CODES=1: no codes, for A/B and tests)
+        char* codes = nullptr;
+        if (!is_set && dc.nbins <= 255 && cd.nrecord_ids <= nrec && !(dc.flags & COL_BROKEN) && !getenv("SG_NO_CODES")) {
+          const int rc = code_alloc(t, align_up(nrec, 16), &codes);
+          if (rc != SG_OK) return rc;
+          enc_bytes += (int64_t)align_up(nrec, 16);
+        }
+        if (codes || (cd.nrecord_ids == nrec && !is_set)) {
+          stats_slots.push_back((uint32_t)cd.col_slot);
+          stats_codes.push_back((unsigned long long)(uintptr_t)codes);
+        }
       }
     } else if (cd.encoding == SG_ENC_VALUES) {
       dc.nitems = cd.nvalues;
@@ -966,6 +1009,7 @@ static int add_block_impl(sg_table* t, const sg_block_desc* b, const Premap& pm)
           if (val_size != 8) dc.vbase = cd.value_base;
           t->has_values_int[(size_t)cd.col_slot] = 1;
           stats_slots.push_back((uint32_t)cd.col_slot);
+          stats_codes.push_back(0ull);
         }
         tm.has_data = true;
       }
@@ -1091,6 +1135,7 @@ static int add_block_impl(sg_table* t, const sg_block_desc* b, const Premap& pm)
   for (int i = 0; i < b->ninfo; i++) hb.info.push_back(b->info[i]);
   t->blocks.push_back(std::move(hb));
   for (uint32_t sl : stats_slots) t->pending_stats.push_back((uint32_t)(t->blocks.size() - 1) * (uint32_t)t->ncols + sl);
+  t->pending_codes.insert(t->pending_codes.end(), stats_codes.begin(), stats_codes.end());
   t->cols.insert(t->cols.end(), dcs.begin(), dcs.end());
   t->total_rows += nrec;
   t->encoded_bytes += enc_bytes;
@@ -1179,9 +1224,12 @@ int sg_table_clear(sg_table* t) {
   t->cols.clear();
   t->segs.clear();
   t->pending_stats.clear();
+  t->pending_codes.clear();
   for (auto& vh : t->vhash) vh.blocks_done = 0;
   t->chunk_idx = 0;
   t->chunk_used = 0;
+  t->code_idx = 0;
+  t->code_used = 0;
   t->stage[0].pending = t->stage[1].pending = false;
   t->stage[0].used = t->stage[1].used = 0;
   t->total_rows = 0;
@@ -1514,9 +1562,13 @@ int upload_table(sg_table* t) {
     // arrays from HBM, once per staging): they select the 32-bit / check-free kernel paths
     uint32_t* d_items = nullptr;
     size_t n = t->pending_stats.size();
-    CUDA_TRY(c, pool_alloc(c, (void**)&d_items, n * 4));
+    // items (u32) then, 8-byte aligned, where each item's codes go
+    const size_t codes_off = align_up(n * 4, 8);
+    CUDA_TRY(c, pool_alloc(c, (void**)&d_items, codes_off + n * 8));
+    const unsigned long long* d_codes = reinterpret_cast<const unsigned long long*>(reinterpret_cast<char*>(d_items) + codes_off);
     CUDA_TRY(c, cudaMemcpyAsync(d_items, t->pending_stats.data(), n * 4, cudaMemcpyHostToDevice, c->stream));
-    int rc = w16::launch_stats(t->d_cols, t->d_blocks, d_items, (uint32_t)n, (uint32_t)t->ncols, c->stream);
+    CUDA_TRY(c, cudaMemcpyAsync((void*)d_codes, t->pending_codes.data(), n * 8, cudaMemcpyHostToDevice, c->stream));
+    int rc = w16::launch_stats(t->d_cols, t->d_blocks, d_items, d_codes, (uint32_t)n, (uint32_t)t->ncols, c->stream);
     if (rc != 0) {
       c->set_err(std::string("stats kernel launch: ") + cudaGetErrorString((cudaError_t)rc));
       pool_release(c, d_items);
@@ -1526,6 +1578,7 @@ int upload_table(sg_table* t) {
     CUDA_TRY(c, cudaMemcpy(t->cols.data(), t->d_cols, nb * (size_t)t->ncols * sizeof(DevCol), cudaMemcpyDeviceToHost));
     pool_release(c, d_items);
     t->pending_stats.clear();
+    t->pending_codes.clear();
     t->stats_launches++;
   }
   t->dirty = false;
@@ -2451,10 +2504,22 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list) {
         const DevCol& dc = t->cols[(size_t)b * (size_t)t->ncols + (size_t)P.groups[0].col];
         count_bins += dc.enc == SG_ENC_BUCKET && (dc.flags & COL_FULL) ? 1u : 0u;
       }
+    // codes: plan columns (filters, groups, the time column, aggregations) with per-row codes (COL_CODES) in some listed block
+    std::vector<int32_t> pcols;
+    for (int i = 0; i < P.nfilters; i++) pcols.push_back(P.filters[i].col);
+    for (int i = 0; i < P.ngroups; i++) pcols.push_back(P.groups[i].col);
+    if (P.time_col >= 0) pcols.push_back(P.time_col);
+    for (int i = 0; i < P.naggs; i++) pcols.push_back(P.aggs[i].col);
+    uint32_t ncodes = 0;
+    for (int32_t col : pcols) {
+      bool any = false;
+      for (uint32_t b : list) any = any || (t->cols[(size_t)b * (size_t)t->ncols + (size_t)col].flags & COL_CODES) != 0u;
+      ncodes += any ? 1u : 0u;
+    }
     fprintf(stderr, "sg_plan: build=%s slot_bytes=%u acc_repl=%u fold_every=%u fail_mode=%u hist_rows=%u lslots=%u nslots=%u hashed=%d"
-            " hashg=%d gbits=%u fbits=%d tbit=%d count_bins=%u",
+            " hashg=%d gbits=%u fbits=%d tbit=%d count_bins=%u codes=%u",
             q->variant->name, q->slot_bytes, P.acc_repl, lp.fold_every, P.fail_mode, P.hist_rows, P.lslots, P.nslots,
-            q->hashed ? 1 : 0, q->hashg ? 1 : 0, P.gbits, __builtin_popcount(P.filt_mask), P.time_ok ? 1 : 0, count_bins);
+            q->hashed ? 1 : 0, q->hashg ? 1 : 0, P.gbits, __builtin_popcount(P.filt_mask), P.time_ok ? 1 : 0, count_bins, ncodes);
     for (int i = 0; i < P.nfilters; i++) {  // per set filter: the most segments its column has in a listed block
       if (P.filters[i].op != SG_OP_IN && P.filters[i].op != SG_OP_NIN) continue;
       uint32_t segs = 0;
