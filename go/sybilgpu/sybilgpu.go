@@ -237,6 +237,10 @@ type Query struct {
 	TimeMax    int64
 	WeightSlot int32 // OPTS.WEIGHT_COL_ID, -1: unweighted (a zero-valued Query must set -1 explicitly)
 	StrReplace []StrReplaced // OPTS.STR_REPLACEMENTS, one entry per rewritten str column
+
+	// Rows without the weight column take the weight of the block's previous row that has it (1 if none), as
+	// LoadAndQueryRecords does.  False: such a row fails the query with SG_ERR_UNSUPPORTED at finish.
+	WeightCarry bool
 }
 
 // StrReplaced carries, for one str column, the rewritten text of every string of its global dictionary
@@ -300,7 +304,10 @@ func (t *Table) Run(q *Query, allreduce bool) (*C.sg_result, error) {
 	d.filters, d.groups, d.aggs = fl, gr, ag
 	d.time_col_slot, d.time_bucket = C.int32_t(q.TimeSlot), C.int64_t(q.TimeBucket)
 	d.time_min, d.time_max = C.int64_t(q.TimeMin), C.int64_t(q.TimeMax)
-	d.weight_col_slot = C.int32_t(q.WeightSlot) // -1: unweighted; rows without the column: SG_ERR_UNSUPPORTED at finish
+	d.weight_col_slot = C.int32_t(q.WeightSlot) // -1: unweighted
+	if q.WeightCarry { // rows without the column reuse the previous row's weight; else SG_ERR_UNSUPPORTED at finish
+		d.weight_carry = 1
+	}
 	// SortResults(OrderBy, OrderAsc) and FLAGS.LIMIT (ABI v2)
 	d.order_by_agg = C.SG_ORDER_COUNT
 	if spec.OrderBy == "" {

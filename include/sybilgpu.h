@@ -130,15 +130,22 @@ typedef struct sg_query_desc {
   int64_t time_max;        /*   dense time-bucket axis (rows outside are counted in overflow) */
   int32_t weight_col_slot; /* OPTS.WEIGHT_COL_ID, -1 = unweighted.  Count / hist Count / bucket counters / sums are
                             * weighted, Samples and MatchedCount count rows (aggregate.go:100-102,202-203).  A scanned
-                            * row WITHOUT the column fails the query at sg_query_finish (SG_ERR_UNSUPPORTED): the
-                            * reference reuses the previous row's weight there */
+                            * row WITHOUT the column (an unlisted row of a bucket column, a row past a short value
+                            * array, a block without the file) is what weight_carry decides */
   /* SortResults (aggregate.go:43-54,497-525): QuerySpec.OrderBy = "$COUNT" (SG_ORDER_COUNT), the name of an
    * aggregation (its index: groups ordered by Hists[col].Mean(), descending) or "" (SG_ORDER_NONE: no sort,
    * groups come in slot order); OrderAsc reverses the sorted list.  Ties (Go's sort is unstable): GroupByKey
    * ascending before the reversal.  A group without the histogram sorts as mean = -inf (Go would panic). */
   int32_t order_by_agg;
   int32_t order_asc;
-  int32_t _pad;
+  /* Rows without the weight column of a weighted query (weight_col_slot >= 0; ignored otherwise):
+   *   0 = the query fails at sg_query_finish with SG_ERR_UNSUPPORTED when a scanned row lacks the column;
+   *   1 = such a row takes the weight of the nearest earlier row of its block that has the column, or 1 when
+   *       none does (aggregate.go:68,100-102: `weight` starts at 1 per block and is overwritten by every row
+   *       holding the column, before the filters run).  Blocks never carry into each other.  This is what
+   *       LoadAndQueryRecords computes.
+   * Any other value is SG_ERR_INVALID. */
+  int32_t weight_carry;
   /* FLAGS.LIMIT (printer.go): > 0 = only the first `limit` groups of the sorted list are materialised
    * (sg_result_num_groups); Cumulative and sg_result_num_groups_total still cover every group.  0 = all. */
   int64_t limit;

@@ -49,7 +49,7 @@ class sg_query_desc(C.Structure):
                 ("hist_bucket", C.c_int32), ("nfilters", C.c_int32), ("ngroups", C.c_int32), ("naggs", C.c_int32),
                 ("time_col_slot", C.c_int32), ("time_bucket", C.c_int64), ("time_min", C.c_int64),
                 ("time_max", C.c_int64), ("weight_col_slot", C.c_int32), ("order_by_agg", C.c_int32),
-                ("order_asc", C.c_int32), ("_pad", C.c_int32), ("limit", C.c_int64),
+                ("order_asc", C.c_int32), ("weight_carry", C.c_int32), ("limit", C.c_int64),
                 ("filters", C.POINTER(sg_filter_desc)), ("groups", C.POINTER(sg_group_desc)),
                 ("aggs", C.POINTER(sg_agg_desc))]
 

@@ -69,6 +69,13 @@ struct DevCol {
 };
 static_assert(sizeof(DevCol) == 80, "DevCol layout");
 
+// A block's weight column leaves rows of its nrec rows unlisted, so they carry an earlier row's weight: a bucket
+// column not checked to list every row, or a value array shorter than the block.  An absent column lists no row:
+// every row keeps weight 1 without a carry.
+__host__ __device__ static inline bool weight_needs_carry(const DevCol& c, uint32_t nrec) {
+  return (c.enc == SG_ENC_BUCKET && !(c.flags & COL_FULL)) || (c.enc == SG_ENC_VALUES && c.nitems < nrec);
+}
+
 struct DevBlock {
   int64_t block_index;
   uint32_t num_records;
@@ -159,6 +166,8 @@ struct Plan {
   uint32_t fail_mode;   // filters set a sticky FAIL bit (finc) instead of counting passes: every filter column
                         // of every listed block populates every row (value array, or a bucket column with
                         // COL_FULL), so only the FAILING bins of a bucket column need to be walked
+  uint32_t wcarry;      // weighted query with sg_query_desc.weight_carry: a row without the weight column (digit
+                        // 0 on the last group axis) takes the digit of the nearest earlier row of its block
   // ---- slot window.  The slot words, the replicated accumulators and the histogram cache index a
   // LOCAL slot space: the group part plus a block-relative time code (1..time_win; 0 = no time).  The
   // global slot of local slot l is l + tbase, tbase = (first time code of the block - 1) * time_stride

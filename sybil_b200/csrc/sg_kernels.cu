@@ -1255,6 +1255,51 @@ __device__ __noinline__ void agg_slow(const AggSlow* A, uint32_t g, long long v,
   if (A->nsub > 0) hist_bucket_general(A, g, v);
 }
 
+// Weights carried over rows without the weight column (Plan::wcarry; aggregate.go:68,100-102).  After the group
+// passes such a row's digit on the weight axis (the last group axis: stride, radix) is 0; it takes the digit of the
+// nearest earlier row of the block whose digit is not 0, or keeps 0 (weight 1) when there is none.  That is a
+// "last non-zero" scan over the block's rows.  Each warp owns a contiguous run of rows: it finds its run's last
+// non-zero digit walking back from the end (one 32-row step unless the run's tail lacks the column), the warps
+// exchange those once through `xw` (NWARPS words of shared memory), and each warp then walks its run forward
+// 32 rows a step, a ballot and two shuffles per step.  Every digit is read back from the slot word, whichever
+// pass wrote it.  Inlined: as an out-of-line call it moved the caller's register allocation (spill loads of the
+// shared-accumulator instantiations +260 bytes, the C3 bench kernel 0.2% slower on H100); inlined, the unweighted
+// instantiations spill within 20 bytes of what they did without it.
+template <typename SlotT>
+__device__ __forceinline__ void carry_weight(SlotT* slot, uint32_t nrec, uint32_t gmask, uint32_t stride, uint32_t radix,
+                                          uint32_t* xw) {
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  const uint32_t per = (nrec + 32u * NWARPS - 1u) / (32u * NWARPS) * 32u;  // rows per warp, whole steps
+  const uint32_t r0 = min(warp * per, nrec), r1 = min(r0 + per, nrec);
+  auto digit = [&](uint32_t r) -> uint32_t { return r < r1 ? (((uint32_t)slot[r] & gmask) / stride) % radix : 0u; };
+  uint32_t last = 0;
+  if (r1 > r0) {
+    for (uint32_t b = r0 + (r1 - 1u - r0) / 32u * 32u;; b -= 32u) {
+      const uint32_t d = digit(b + lane);
+      const uint32_t m = __ballot_sync(FULL, d != 0u);
+      if (m) {
+        last = __shfl_sync(FULL, d, 31 - __clz(m));
+        break;
+      }
+      if (b == r0) break;
+    }
+  }
+  if (lane == 0) xw[warp] = last;
+  __syncthreads();
+  uint32_t carry = 0;
+  for (uint32_t w = 0; w < warp; w++)
+    if (xw[w]) carry = xw[w];
+  for (uint32_t b = r0; b < r1; b += 32u) {
+    const uint32_t r = b + lane, d = digit(r);
+    const uint32_t below = __ballot_sync(FULL, d != 0u) & (FULL >> (31u - lane));  // lanes <= this one with a digit
+    const uint32_t src = __shfl_sync(FULL, d, below ? 31 - __clz(below) : 0);
+    const uint32_t v = below ? src : carry;
+    if (d == 0u && v != 0u && r < r1) slot[r] = (SlotT)(slot[r] + v * stride);
+    carry = __shfl_sync(FULL, v, 31);
+  }
+  __syncthreads();
+}
+
 // ---------------------------------------------------------------------------
 // the kernel
 // ---------------------------------------------------------------------------
@@ -2078,6 +2123,14 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
     }
     __syncthreads();
     if (time_pass) pass_mark(pass_no++);
+
+    // ---- weights carried over the block's rows without the weight column (see carry_weight); the group passes
+    // above wrote every row, including rows that already failed a filter, so each row holds its own digit.
+    // (count_in_group needs COL_FULL on its one group column, so it never meets a block that carries.)
+    if (PP->wcarry && weight_needs_carry(colcache[nfilters + ngroups - 1], nrec)) {
+      const KGroup& WG = PP->groups[ngroups - 1];
+      carry_weight<SlotT>(slot, nrec, gmask, WG.stride, WG.radix, cx.binpay_s);
+    }
 
     // ---- hashed slot space (LaunchParams::hkeys): code -> index of an open-addressing table in global memory.
     // Only rows that passed every filter (and carry a time code in time mode) take a slot.  The reference keys a Go

@@ -1738,10 +1738,13 @@ int make_plan(sg_query* q, const std::vector<uint32_t>& list) {
   // Weighted queries (OPTS.WEIGHT_COL, aggregate.go:68,100-102,202-203; hist_basic.go:111-151): Count += weight,
   // hist Count += weight, Values[bucket] += weight, mean weighted.  All of these are linear in the weight, so the
   // scan groups by the weight VALUE as one more (hidden, last) axis — the ordinary int group-by — and the host
-  // folds that axis away with a multiplication per slot (fold_axes).  Rows WITHOUT the weight column would reuse
-  // the previous row's weight in the reference (Q13): such a query is refused when the result is built.
+  // folds that axis away with a multiplication per slot (fold_axes).  Rows WITHOUT the weight column reuse the
+  // previous row's weight in the reference (Q13): with weight_carry the scan fills their digit of the weight axis
+  // forward from the nearest earlier row of the block (a row with no such row keeps code 0: weight 1); without it
+  // such a query is refused when the result is built.
   q->pgroups = q->groups;
   const bool weighted = q->d.weight_col_slot >= 0;
+  P.wcarry = weighted && q->d.weight_carry == 1 ? 1u : 0u;
   if (weighted) {
     if (q->d.weight_col_slot >= t->ncols || t->types[(size_t)q->d.weight_col_slot] != SG_COL_INT) {
       c->set_err("query: the weight column must be an int column");
@@ -2516,10 +2519,17 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list) {
       for (uint32_t b : list) any = any || (t->cols[(size_t)b * (size_t)t->ncols + (size_t)col].flags & COL_CODES) != 0u;
       ncodes += any ? 1u : 0u;
     }
+    // wcarry: listed blocks whose weight column the kernel fills forward over unlisted rows
+    uint32_t wcarry = 0;
+    if (P.wcarry)
+      for (uint32_t b : list)
+        wcarry += weight_needs_carry(t->cols[(size_t)b * (size_t)t->ncols + (size_t)P.groups[P.ngroups - 1].col],
+                                     (uint32_t)t->blocks[b].num_records) ? 1u : 0u;
     fprintf(stderr, "sg_plan: build=%s slot_bytes=%u acc_repl=%u fold_every=%u fail_mode=%u hist_rows=%u lslots=%u nslots=%u hashed=%d"
-            " hashg=%d gbits=%u fbits=%d tbit=%d count_bins=%u codes=%u",
+            " hashg=%d gbits=%u fbits=%d tbit=%d count_bins=%u codes=%u wcarry=%u",
             q->variant->name, q->slot_bytes, P.acc_repl, lp.fold_every, P.fail_mode, P.hist_rows, P.lslots, P.nslots,
-            q->hashed ? 1 : 0, q->hashg ? 1 : 0, P.gbits, __builtin_popcount(P.filt_mask), P.time_ok ? 1 : 0, count_bins, ncodes);
+            q->hashed ? 1 : 0, q->hashg ? 1 : 0, P.gbits, __builtin_popcount(P.filt_mask), P.time_ok ? 1 : 0, count_bins, ncodes,
+            wcarry);
     for (int i = 0; i < P.nfilters; i++) {  // per set filter: the most segments its column has in a listed block
       if (P.filters[i].op != SG_OP_IN && P.filters[i].op != SG_OP_NIN) continue;
       uint32_t segs = 0;
@@ -2981,7 +2991,9 @@ static int build_result_topk(sg_query* q, sg_result** out, bool* fell_back) {
 // Weights (OPTS.WEIGHT_COL): the scan grouped by the weight value as a hidden last axis (make_plan); the slots of
 // weight w are multiplied by w and added onto code 0 of that axis — Count / hist Count / Values[] += weight
 // (aggregate.go:203, hist_basic.go:111-116,146), exact sum += value * weight; Result.Samples keeps the rows.
-// A row without the weight column would reuse the previous row's weight (Q13, aggregate.go:68,100-102): refused.
+// A row without the weight column reuses the previous row's weight (Q13, aggregate.go:68,100-102).  With
+// weight_carry the scan has already given such a row that weight's code, and a row left on code 0 had no earlier
+// row with the column in its block: weight 1, so the slot stays in place.  Without weight_carry it is refused.
 static int fold_axes(sg_query* q, uint64_t* h, size_t have, sg_result* r, int64_t* matched_rows) {
   const Plan& P = q->plan;
   sg_ctx* c = q->ctx;
@@ -3004,7 +3016,7 @@ static int fold_axes(sg_query* q, uint64_t* h, size_t have, sg_result* r, int64_
       for (uint32_t s = 0; s < P.nslots; s++) {
         if (!cnt[s]) continue;
         const uint32_t code = (s / d.stride) % d.radix;
-        if (code == 0) {
+        if (code == 0 && !P.wcarry) {
           c->set_err("query: rows without the weight column (the reference reuses the previous row's weight, "
                      "aggregate.go:68,100-102): not reproduced by this engine");
           return SG_ERR_UNSUPPORTED;
@@ -3365,6 +3377,10 @@ sg_query* sg_query_begin(sg_ctx* c, sg_table* t, const sg_query_desc* d) {
   if (d->nfilters < 0 || d->nfilters > SG_MAX_FILTERS || d->ngroups < 0 || d->ngroups > SG_MAX_GROUPS ||
       d->naggs < 0 || d->naggs > SG_MAX_AGGS) {
     c->set_err("sg_query_begin: too many filters / groups / aggregations for this build");
+    return nullptr;
+  }
+  if (d->weight_carry != 0 && d->weight_carry != 1) {
+    c->set_err("sg_query_begin: weight_carry must be 0 or 1");
     return nullptr;
   }
   if (!t) {

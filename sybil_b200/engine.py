@@ -36,6 +36,10 @@ class _Flags:
         self.TIME_BUCKET = 0
         self.LIMIT = 100
         self.WEIGHT_COL = ""  # config.go:81; OPTS.WEIGHT_COL / WEIGHT_COL_ID follow from it (cmd_query.go:317-320)
+        # The engine's own flag, not one of config.go: rows without the weight column take the weight of the block's
+        # previous row that has it, as LoadAndQueryRecords does (sg_query_desc.weight_carry).  False: a weighted
+        # query over such rows fails with SG_ERR_UNSUPPORTED.
+        self.WEIGHT_CARRY = False
 
 
 FLAGS = _Flags()
@@ -330,6 +334,7 @@ def make_query_desc(KeyTable, KeyTypes, IntInfo, qs):
     d.groups = C.cast(gr, C.POINTER(F.sg_group_desc))
     d.aggs = C.cast(ag, C.POINTER(F.sg_agg_desc))
     d.weight_col_slot = KeyTable[FLAGS.WEIGHT_COL] if FLAGS.WEIGHT_COL else -1
+    d.weight_carry = 1 if FLAGS.WEIGHT_CARRY else 0
     # SortResults(OrderBy, OrderAsc) (aggregate.go:497-525)
     order = getattr(qs, "OrderBy", "$COUNT")
     if order == "$COUNT":
