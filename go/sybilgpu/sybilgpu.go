@@ -241,6 +241,9 @@ type Query struct {
 	// Rows without the weight column take the weight of the block's previous row that has it (1 if none), as
 	// LoadAndQueryRecords does.  False: such a row fails the query with SG_ERR_UNSUPPORTED at finish.
 	WeightCarry bool
+	// A group-by whose accumulators would pass 24 GiB keeps accumulators for the groups that occur only, as sybil's
+	// result map does (sg_query_set_sparse_groups).  False: such a query fails with SG_ERR_UNSUPPORTED.
+	SparseGroups bool
 }
 
 // StrReplaced carries, for one str column, the rewritten text of every string of its global dictionary
@@ -328,6 +331,9 @@ func (t *Table) Run(q *Query, allreduce bool) (*C.sg_result, error) {
 		return nil, t.c.err()
 	}
 	defer C.sg_query_free(h)
+	if q.SparseGroups && C.sg_query_set_sparse_groups(h, 1) != C.SG_OK {
+		return nil, t.c.err()
+	}
 	for i, f := range q.Filters {
 		if f.Lut != nil {
 			n := C.sg_table_dict_size(t.h, C.int32_t(f.Slot))

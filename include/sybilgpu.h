@@ -32,7 +32,10 @@ extern "C" {
 
 /* limits of one query (reference has none; beyond these -> SG_ERR_UNSUPPORTED).  Group keys: the product of the
  * group columns' distinct-value counts (x time buckets) may reach 2^31; up to 2^26 it is a dense array, beyond that
- * a hash table on the device keyed by the combined code (single GPU; at most 2^25 distinct groups per query). */
+ * a hash table on the device keyed by the combined code (single GPU; at most 2^25 distinct groups per query).
+ * Accumulators (count, sums, histogram counters per slot of that array or table) may take up to 24 GiB; with
+ * sg_query_set_sparse_groups(q, 1) a plan past that holds accumulators for the groups that occur only, and the
+ * 24 GiB limit applies to those (single GPU, sg_query_run only, no weights or StrReplace). */
 #define SG_MAX_FILTERS 15
 #define SG_MAX_GROUPS 8
 #define SG_MAX_AGGS 16
@@ -290,6 +293,16 @@ int sg_query_set_str_lut(sg_query* q, int32_t filter_index, const uint32_t* bits
  * (EQ "x" = RE bitset of the strings that rewrite to "x").  Call between sg_query_begin and sg_query_finish;
  * n == 0 removes the rewrite.  Not combinable with a cross-GPU merge over differing dictionaries. */
 int sg_query_set_str_replace(sg_query* q, int32_t col_slot, const char* bytes, const uint32_t* offsets, int64_t n);
+/* Sparse group accumulators (the Go reference's result map holds only the groups that occur, aggregate.go:186-203).
+ *   0 (default) = a plan whose accumulators pass 24 GiB (groups x histogram counters) fails with SG_ERR_UNSUPPORTED;
+ *   1 = such a plan scans twice: a discovery pass collects the group keys of every row that passes into a table on
+ *       the device and numbers them, then the aggregation pass accumulates into arrays sized by those L live
+ *       groups, and only those are read back.  It fails with SG_ERR_UNSUPPORTED when the L groups' accumulators
+ *       pass 24 GiB, for weighted queries and StrReplace, and under sg_query_allreduce.  Plans within the limit
+ *       run as with 0.  The streaming path needs every block staged before the first pass: sg_query_submit_block
+ *       fails with SG_ERR_UNSUPPORTED while the setting is 1.
+ * Any other value is SG_ERR_INVALID.  Takes effect at the next sg_query_run (a prepared query plans again). */
+int sg_query_set_sparse_groups(sg_query* q, int32_t on);
 /* ShouldLoadBlockFromDir (table_block_io.go:110-182): 1 = load, 0 = pruned */
 int sg_query_should_load(sg_query* q, const sg_block_desc* block);
 /* Resident path: run the scan over every staged block of the table

@@ -212,9 +212,18 @@ struct LaunchParams {
   // Hashed slot space (group-by products beyond the dense 2^26 slots): after the group / time passes a row's
   // mixed-radix code (< 2^31) is looked up / inserted in this open-addressing table (key = code + 1, 0 = empty) and the
   // slot word's group bits are replaced by the table index, which is what the accumulators are indexed by
-  // (plan.nslots == hmask + 1).  nullptr: the slot space is dense.  scalars[4] counts rows that found the table full.
+  // (plan.nslots == hmask + 1; a sparse plan's accumulators are indexed by hids below, plan.nslots == its live groups,
+  // and the table has hmask + 1 entries all the same).  nullptr: the slot space is dense.  scalars[4] counts rows that
+  // found the table full.
   uint32_t* hkeys;
   uint32_t hmask;
+  // Sparse group accumulators (sg_query_set_sparse_groups): the same table is filled by a discovery launch
+  // (hdisc = 1: codes are inserted, nothing is counted or aggregated), then each occupied entry gets a dense id
+  // (assign_ids), then the aggregation launch (hids != nullptr) looks every code up without inserting and writes
+  // hids[index] into the slot word's group bits.  The accumulators are indexed by that id.  scalars[5] counts rows
+  // whose code the aggregation launch did not find (an internal inconsistency that fails the query).
+  const uint32_t* hids;
+  uint32_t hdisc;
 };
 __host__ __device__ static inline uint32_t slot_hash(uint32_t x) {
   x ^= x >> 16;

@@ -1590,7 +1590,8 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
     if (done) break;
     phase(6);
     const uint32_t bid = item.x, imask = item.y, nrec = item.z;
-    const uint32_t aggmask = imask & 0xffffu;
+    // (a discovery launch of the sparse path aggregates nothing: no aggregation pass enters the block's pass list)
+    const uint32_t aggmask = (sizeof(SlotT) == 4 && lp.hdisc) ? 0u : imask & 0xffffu;
     const bool owner = (imask >> 31) != 0;
     const DevCol* __restrict__ cols = lp.cols + (size_t)bid * ncolslots;
 
@@ -2138,24 +2139,43 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
     if (sizeof(SlotT) == 4 && lp.hkeys != nullptr) {
       uint32_t* const hk = lp.hkeys;
       const uint32_t hmask = lp.hmask;
+      const uint32_t* const hids = lp.hids;
       for (uint32_t r = cx.tid; r < nrec; r += THREADS) {
         const uint32_t s = (uint32_t)slot[r];
         if ((s >> gbits) != pass_target) continue;
         const uint32_t key = (s & gmask) + 1u;
         uint32_t idx = slot_hash(key) & hmask, probes = 0;
-        for (;;) {
-          const uint32_t old = atomicCAS(hk + idx, 0u, key);
-          if (old == 0u || old == key) break;
-          idx = (idx + 1u) & hmask;
-          if (++probes > hmask) {  // table full: the host fails the query (scalars[4])
-            gred_add(g_scalars + 4, 1ull);
-            idx = 0u;
-            break;
+        if (hids != nullptr) {
+          // sparse aggregation launch: the table is complete and read-only; the accumulators are indexed by id
+          for (;;) {
+            const uint32_t k = __ldg(hk + idx);
+            if (k == key) {
+              idx = __ldg(hids + idx);
+              break;
+            }
+            if (k == 0u || ++probes > hmask) {  // not discovered: the host fails the query (scalars[5])
+              gred_add(g_scalars + 5, 1ull);
+              idx = 0u;
+              break;
+            }
+            idx = (idx + 1u) & hmask;
+          }
+        } else {
+          for (;;) {
+            const uint32_t old = atomicCAS(hk + idx, 0u, key);
+            if (old == 0u || old == key) break;
+            idx = (idx + 1u) & hmask;
+            if (++probes > hmask) {  // table full: the host fails the query (scalars[4])
+              gred_add(g_scalars + 4, 1ull);
+              idx = 0u;
+              break;
+            }
           }
         }
         slot[r] = (SlotT)((s & ~gmask) | idx);
       }
       __syncthreads();
+      if (lp.hdisc) continue;  // discovery launch: the table is all it fills
     }
 
     phase(3);

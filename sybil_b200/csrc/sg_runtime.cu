@@ -1426,7 +1426,15 @@ struct sg_query {
   bool hashed = false;
   uint64_t code_space = 0;  // product of the axes' radices
   uint32_t* d_hkeys = nullptr;
+  uint32_t hcap = 0;              // entries of the device table (LaunchParams::hkeys)
   std::vector<uint32_t> h_hkeys;  // read back for the result: slot -> code + 1 (0: empty)
+  // sparse group accumulators (sg_query_set_sparse_groups): a hashed plan whose table is filled by a discovery
+  // launch first; the accumulators then hold the live groups only, indexed by the dense id of their table entry
+  int32_t sparse_req = 0;        // the setter's value, applied by the next plan
+  bool sparse = false;           // this plan takes the path
+  uint32_t* d_hids = nullptr;    // [hcap] table entry -> dense id, then [hcap] dense id -> key (code + 1)
+  uint64_t* d_disc = nullptr;    // the discovery launch's scalars (SCALAR_WORDS), then the live group count
+  double disc_ms = 0;            // the last discovery launch (SG_PLAN_TRACE)
   // accumulators as read back right behind the kernel (small plans): spares build_result a blocking copy
   std::vector<uint64_t> h_acc;
   bool h_acc_valid = false;
@@ -1469,6 +1477,10 @@ void free_device(sg_query* q) {
   pool_release(c, q->d_gslots);
   pool_release(c, q->d_hkeys);
   q->d_hkeys = nullptr;
+  pool_release(c, q->d_hids);
+  q->d_hids = nullptr;
+  pool_release(c, q->d_disc);
+  q->d_disc = nullptr;
   pool_release(c, q->d_gbinpay);
   pool_release(c, q->d_gdummy);
   for (auto p : q->d_luts) pool_release(c, p);
@@ -1682,6 +1694,14 @@ int ensure_value_dict(sg_table* t, int col) {
 // scalars: [0] matched rows, [1] broken blocks, [2] time overflow rows (kernel); [8..15] the cross-GPU
 // merge header (block counters + axes signature) written by sg_query_allreduce
 constexpr size_t SCALAR_WORDS = 16;
+constexpr uint64_t ACC_LIMIT_BYTES = (uint64_t)24 << 30;
+// bytes of the SUM region (scalars | count | sums | hist Counts | bucket counters) for nslots slots: what the
+// 24 GiB limit of layout_accumulators is taken on
+static uint64_t sum_region_bytes(const sg_query* q, uint64_t nslots) {
+  uint64_t per_slot = 1 + 2 * (uint64_t)q->layouts.size();
+  for (const auto& L : q->layouts) per_slot += L.nvals_total;
+  return (SCALAR_WORDS + nslots * per_slot) * 8;
+}
 int layout_accumulators(sg_query* q, uint32_t nslots) {
   const int naggs = (int)q->layouts.size();
   size_t words = SCALAR_WORDS;  // scalars
@@ -1705,8 +1725,9 @@ int layout_accumulators(sg_query* q, uint32_t nslots) {
   for (int i = 0; i < naggs; i++) {
     q->off_buckets.push_back(words);
     words += (size_t)nslots * q->layouts[(size_t)i].nvals_total;
-    if (words * 8 > ((size_t)24 << 30)) {
-      q->ctx->set_err("query: accumulators exceed 24 GiB (groups x histogram buckets); needs the sparse path");
+    if (words * 8 > ACC_LIMIT_BYTES) {
+      q->ctx->set_err("query: accumulators exceed 24 GiB (groups x histogram buckets); needs sparse group "
+                      "accumulators (sg_query_set_sparse_groups)");
       return SG_ERR_UNSUPPORTED;
     }
   }
@@ -1855,24 +1876,71 @@ int make_plan(sg_query* q, const std::vector<uint32_t>& list) {
     stride *= P.time_radix;
   }
   P.nslots = (uint32_t)stride;
+
+  // ---- aggregations ----------------------------------------------------------------
+  // accumulator layout: one SUM region (scalars | count | per agg hcount, sum | per agg buckets)
+  // followed by one MAX region (per agg vmax): the cross-GPU merge is two all-reduces
+  q->layouts.clear();
+  for (int i = 0; i < P.naggs; i++) {
+    const sg_agg_desc& a = q->aggs[(size_t)i];
+    if (!col_ok(a.col_slot)) {
+      c->set_err("query: aggregation column out of range");
+      return SG_ERR_INVALID;
+    }
+    HistLayout L;
+    if (!make_layout(a.info_min, a.info_max, P.hist_mode != 0, q->d.hist_kind == SG_HIST_MULTI, q->d.hist_bucket, L)) {
+      c->set_err("query: IntInfo extents give no usable histogram layout");
+      return SG_ERR_INVALID;
+    }
+    q->layouts.push_back(L);
+    KAgg& ka = P.aggs[i];
+    ka.col = a.col_slot;
+    ka.info_min = a.info_min;
+    ka.info_max = a.info_max;
+    ka.reject_hi = wmul10(a.info_max);
+    ka.nsub = (int32_t)L.subs.size();
+    ka.multi = q->d.hist_kind == SG_HIST_MULTI ? 1u : 0u;
+    ka.nvals_total = L.nvals_total;
+    for (size_t s = 0; s < L.subs.size(); s++) ka.sub[s] = L.subs[s];
+  }
+
   // ---- hashed slot space: more codes than dense slots.  The table gets twice as many entries as rows can make
   // groups (every scanned row its own group at worst), within [2^16, 2^26]; a table that fills up fails the query.
   q->code_space = stride;
   // tests: SG_FORCE_HASHED_SLOTS=1 takes the hashed slot space at any size (it must give what the dense one gives);
   // SG_HASH_CAP_LOG2=n caps its table at 2^n entries, so that a table that fills up can be reached with few rows
-  q->hashed = (stride > (uint64_t)MAX_SLOTS || getenv("SG_FORCE_HASHED_SLOTS")) && !getenv("SG_NO_HASHED_SLOTS");
-  if (stride > (uint64_t)MAX_SLOTS && !q->hashed) {
-    c->set_err("query: group-by cardinality product exceeds the dense slot space");
-    return SG_ERR_UNSUPPORTED;
-  }
-  if (q->hashed) {
+  bool hashed = (stride > (uint64_t)MAX_SLOTS || getenv("SG_FORCE_HASHED_SLOTS")) && !getenv("SG_NO_HASHED_SLOTS");
+  uint64_t cap = 0;
+  {
     uint64_t rows = 0;
     for (uint32_t b : list) rows += t->blocks[b].num_records;
     uint64_t cap_max = (uint64_t)MAX_SLOTS;
     if (const char* e = getenv("SG_HASH_CAP_LOG2")) cap_max = (uint64_t)1 << std::min(std::max(atoi(e), 4), 26);
-    uint64_t cap = std::min<uint64_t>((uint64_t)1 << 16, cap_max);
+    cap = std::min<uint64_t>((uint64_t)1 << 16, cap_max);
     while (cap < 2 * std::min<uint64_t>(rows, stride) && cap < cap_max) cap <<= 1;
+  }
+  // ---- sparse group accumulators (sg_query_set_sparse_groups): a plan whose accumulators, dense or hashed, pass the
+  // 24 GiB limit keys the same table by the row's code, and its accumulators hold only the groups a discovery
+  // launch finds.  Plans within the limit are planned as without the flag.
+  // tests: SG_FORCE_SPARSE_GROUPS=1 takes the sparse path for every plan while the flag is set
+  q->sparse = q->sparse_req == 1 &&
+              (getenv("SG_FORCE_SPARSE_GROUPS") || sum_region_bytes(q, hashed ? cap : stride) > ACC_LIMIT_BYTES);
+  if (q->sparse) {
+    if (weighted || !q->repl.empty()) {
+      c->set_err("query: weights / StrReplace are not combined with sparse group accumulators in this build");
+      return SG_ERR_UNSUPPORTED;
+    }
+    hashed = true;
+  }
+  q->hashed = hashed;
+  if (stride > (uint64_t)MAX_SLOTS && !q->hashed) {
+    c->set_err("query: group-by cardinality product exceeds the dense slot space");
+    return SG_ERR_UNSUPPORTED;
+  }
+  q->hcap = 0;
+  if (q->hashed) {
     P.nslots = (uint32_t)cap;
+    q->hcap = (uint32_t)cap;
   }
   // ---- fail mode: every filter column populates every row of every listed block (value array, or a
   // bucket column whose bins were checked to list each row once) -> one sticky FAIL bit instead of a
@@ -2027,34 +2095,9 @@ int make_plan(sg_query* q, const std::vector<uint32_t>& list) {
     }
   }
 
-  // ---- aggregations ----------------------------------------------------------------
-  // accumulator layout: one SUM region (scalars | count | per agg hcount, sum | per agg buckets)
-  // followed by one MAX region (per agg vmax): the cross-GPU merge is two all-reduces
-  q->layouts.clear();
-  for (int i = 0; i < P.naggs; i++) {
-    const sg_agg_desc& a = q->aggs[(size_t)i];
-    if (!col_ok(a.col_slot)) {
-      c->set_err("query: aggregation column out of range");
-      return SG_ERR_INVALID;
-    }
-    HistLayout L;
-    if (!make_layout(a.info_min, a.info_max, P.hist_mode != 0, q->d.hist_kind == SG_HIST_MULTI, q->d.hist_bucket, L)) {
-      c->set_err("query: IntInfo extents give no usable histogram layout");
-      return SG_ERR_INVALID;
-    }
-    q->layouts.push_back(L);
-    KAgg& ka = P.aggs[i];
-    ka.col = a.col_slot;
-    ka.info_min = a.info_min;
-    ka.info_max = a.info_max;
-    ka.reject_hi = wmul10(a.info_max);
-    ka.nsub = (int32_t)L.subs.size();
-    ka.multi = q->d.hist_kind == SG_HIST_MULTI ? 1u : 0u;
-    ka.nvals_total = L.nvals_total;
-    for (size_t s = 0; s < L.subs.size(); s++) ka.sub[s] = L.subs[s];
-  }
   {
-    int rc = layout_accumulators(q, P.nslots);
+    // sparse plans are laid out for their live groups once the discovery launch has counted them
+    int rc = layout_accumulators(q, q->sparse ? 0u : P.nslots);
     if (rc != SG_OK) return rc;
   }
 
@@ -2207,6 +2250,8 @@ int make_plan(sg_query* q, const std::vector<uint32_t>& list) {
   return SG_OK;
 }
 
+void point_plan(sg_query* q);
+
 int alloc_device(sg_query* q) {
   sg_ctx* c = q->ctx;
   sg_table* t = q->table;
@@ -2235,12 +2280,23 @@ int alloc_device(sg_query* q) {
     CUDA_TRY(c, pool_alloc(c, (void**)&q->d_gslots, grid_cap * SG_BLOCK_ROWS * 4));
   pool_release(c, q->d_hkeys);
   q->d_hkeys = nullptr;
-  if (q->hashed) CUDA_TRY(c, pool_alloc(c, (void**)&q->d_hkeys, (size_t)q->plan.nslots * 4));
+  pool_release(c, q->d_hids);
+  q->d_hids = nullptr;
+  if (q->hashed) CUDA_TRY(c, pool_alloc(c, (void**)&q->d_hkeys, (size_t)q->hcap * 4));
+  if (q->sparse) {
+    CUDA_TRY(c, pool_alloc(c, (void**)&q->d_hids, (size_t)q->hcap * 8));
+    if (!q->d_disc) CUDA_TRY(c, pool_alloc(c, (void**)&q->d_disc, (SCALAR_WORDS + 1) * 8));
+  }
   if (!q->ev0) {
     CUDA_TRY(c, cudaEventCreate(&q->ev0));
     CUDA_TRY(c, cudaEventCreate(&q->ev1));
   }
-  // point the plan at the accumulators
+  point_plan(q);
+  return SG_OK;
+}
+
+// point the plan at the accumulators
+void point_plan(sg_query* q) {
   Plan& P = q->plan;
   P.scalars = q->d_acc;
   P.count = q->d_acc + q->off_count;
@@ -2252,7 +2308,6 @@ int alloc_device(sg_query* q) {
     P.aggs[i].vmin = nullptr;
     P.aggs[i].buckets = q->d_acc + q->off_buckets[(size_t)i];
   }
-  return SG_OK;
 }
 
 // ---- top-K selection on the device (results with very many groups and a limit) ------------------------------
@@ -2364,7 +2419,8 @@ __global__ void fill_i64(int64_t* p, size_t n, int64_t v) {
 int reset_accumulators(sg_query* q) {
   sg_ctx* c = q->ctx;
   CUDA_TRY(c, cudaMemsetAsync(q->d_acc, 0, q->sum_words * 8, c->stream));
-  if (q->hashed && q->d_hkeys) CUDA_TRY(c, cudaMemsetAsync(q->d_hkeys, 0, (size_t)q->plan.nslots * 4, c->stream));
+  // (a sparse plan's table was filled by its discovery launch, which cleared it first)
+  if (q->hashed && !q->sparse && q->d_hkeys) CUDA_TRY(c, cudaMemsetAsync(q->d_hkeys, 0, (size_t)q->hcap * 4, c->stream));
   if (q->acc_words > q->sum_words) {
     size_t n = q->acc_words - q->sum_words;
     fill_i64<<<(unsigned)((n + 255) / 256), 256, 0, c->stream>>>((int64_t*)(q->d_acc + q->sum_words), n, INT64_MIN);
@@ -2374,8 +2430,9 @@ int reset_accumulators(sg_query* q) {
   return SG_OK;
 }
 
-// one launch of the scan kernel over `list`
-int run_list(sg_query* q, const std::vector<uint32_t>& list) {
+// one launch of the scan kernel over `list`.  discover: the discovery launch of a sparse plan (its scalars go to
+// d_disc and are what comes back)
+int run_list(sg_query* q, const std::vector<uint32_t>& list, bool discover = false) {
   sg_ctx* c = q->ctx;
   sg_table* t = q->table;
   // Work items.  The blocks of the last, partial wave (n mod #SMs) would leave most SMs idle for a
@@ -2406,7 +2463,7 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list) {
   // small accumulator arrays come back right behind the scan (build_result then needs no further copy) — unless a
   // cross-GPU merge follows, which reads the MERGED array back itself: then only the scalars (broken blocks) do
   const bool merge_follows = c->comm != nullptr && c->nranks > 1;
-  const size_t acc_back = (!merge_follows && q->acc_words * 8 <= ((size_t)4 << 20)) ? q->acc_words * 8 : 64;
+  const size_t acc_back = (!discover && !merge_follows && q->acc_words * 8 <= ((size_t)4 << 20)) ? q->acc_words * 8 : 64;
   const size_t off_items = (sizeof(Plan) + 255) & ~(size_t)255;
   const size_t off_acc = off_items + ((items.size() * 16 + 255) & ~(size_t)255);
   char* hp = c->scratch(off_acc + acc_back);
@@ -2450,7 +2507,9 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list) {
   lp.dbg = nullptr;
   lp.hashg = q->hashg ? 1u : 0u;
   lp.hkeys = q->hashed ? q->d_hkeys : nullptr;
-  lp.hmask = q->hashed ? q->plan.nslots - 1u : 0u;
+  lp.hmask = q->hashed ? q->hcap - 1u : 0u;
+  lp.hids = q->sparse && !discover ? q->d_hids : nullptr;
+  lp.hdisc = discover ? 1u : 0u;
   // Deferred fold: the replicated 32-bit accumulators of up to fold_every consecutive blocks are
   // folded together.  Needs one encoding per aggregation column across the listed blocks (word0
   // counts accepted rows for bucket columns, rejected ones for value arrays) and keeps the hot
@@ -2497,7 +2556,9 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list) {
     }
   }
   lp.tmaps = lp.stage_units ? t->d_tmaps : nullptr;
-  if (getenv("SG_PLAN_TRACE")) {  // SG_PLAN_TRACE=1: one line per launch on stderr, so a test can see which path it reached
+  // SG_PLAN_TRACE=1: one line per launch on stderr, so a test can see which path it reached (a sparse plan: one per
+  // aggregation launch)
+  if (getenv("SG_PLAN_TRACE") && !discover) {
     const Plan& P = q->plan;
     // (the slot word: gbits group bits, fbits pass-counter / fail and set-filter bits, tbit time bit)
     // count_bins: listed blocks whose group Count the kernel takes from bin sizes (its count_in_group conditions)
@@ -2553,6 +2614,7 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list) {
                                            0x100000000ull;
       fprintf(stderr, " agg%d=[fmin=%lld fmax=%lld hist32=%d nocarry=%d]", a, fmin, fmax, hist32 ? 1 : 0, nocarry ? 1 : 0);
     }
+    if (q->sparse) fprintf(stderr, " sparse=1 live=%u table=%u", P.nslots, q->hcap);
     fprintf(stderr, "\n");
   }
   int grid = (int)std::min<size_t>((size_t)q->grid, std::max<size_t>(items.size(), 1));
@@ -2573,7 +2635,7 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list) {
     if (!q->h_pin) q->h_pin = c->pin_get(acc_back, &q->h_pin_bytes);
   }
   char* const back = to_pin && q->h_pin ? q->h_pin : hp + off_acc;
-  CUDA_TRY(c, cudaMemcpyAsync(back, q->d_acc, acc_back, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(c, cudaMemcpyAsync(back, discover ? q->d_disc : q->d_acc, acc_back, cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(c, cudaStreamSynchronize(c->stream));
   if (back == q->h_pin) {
     q->h_acc.assign((const uint64_t*)back, (const uint64_t*)back + 8);  // the scalars (sg_query_run reads them)
@@ -2587,6 +2649,7 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list) {
   float ms = 0;
   CUDA_TRY(c, cudaEventElapsedTime(&ms, q->ev0, q->ev1));
   q->kernel_ms += ms;
+  if (discover) q->disc_ms = ms;
   q->launches += 1;
   if (d_dbg) {
     std::vector<unsigned long long> hd((size_t)q->grid * 16);
@@ -2608,6 +2671,90 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list) {
               tot[11] / q->grid, tot[12] / q->grid, tot[13] / q->grid, tot[14] / q->grid, tot[15] / q->grid);
     pool_release(c, d_dbg);
   }
+  return SG_OK;
+}
+
+// Dense ids of the sparse path: every occupied entry of the table gets an id in 0..L-1 (in no set order: the result
+// orders its groups itself), id2key[id] = the entry's key (code + 1), *live = L.  One warp-aggregated atomic per warp
+// and step; the launch runs after every insert of the discovery launch is done.
+__global__ void assign_ids(const uint32_t* __restrict__ keys, uint32_t cap, uint32_t* __restrict__ ids,
+                           uint32_t* __restrict__ id2key, unsigned int* live) {
+  const uint32_t stride = gridDim.x * blockDim.x;
+  for (uint32_t base = blockIdx.x * blockDim.x; base < cap; base += stride) {
+    const uint32_t i = base + threadIdx.x;
+    const uint32_t k = i < cap ? keys[i] : 0u;
+    const unsigned m = __ballot_sync(0xffffffffu, k != 0u);
+    if (!m) continue;
+    const int lane = (int)(threadIdx.x & 31u);
+    unsigned first = 0;
+    if (lane == __ffs((int)m) - 1) first = atomicAdd(live, (unsigned)__popc(m));
+    first = __shfl_sync(0xffffffffu, first, __ffs((int)m) - 1);
+    if (k != 0u) {
+      const uint32_t id = first + (uint32_t)__popc(m & ((1u << lane) - 1u));
+      ids[i] = id;
+      id2key[id] = k;
+    }
+  }
+}
+
+// Sparse group accumulators, before the aggregation launch: the discovery launch fills the table with the code of
+// every row that passes, assign_ids numbers the entries, and the accumulators are laid out for the L live groups.
+// Refuses when L groups' accumulators pass 24 GiB (tests: SG_SPARSE_BUDGET_MIB=n lowers that budget); the query's
+// device state stays valid for another run.
+int discover_groups(sg_query* q, const std::vector<uint32_t>& list) {
+  sg_ctx* c = q->ctx;
+  Plan& P = q->plan;
+  CUDA_TRY(c, cudaMemsetAsync(q->d_hkeys, 0, (size_t)q->hcap * 4, c->stream));
+  CUDA_TRY(c, cudaMemsetAsync(q->d_disc, 0, (SCALAR_WORDS + 1) * 8, c->stream));
+  uint64_t* const acc_scalars = P.scalars;
+  P.scalars = q->d_disc;
+  int rc = run_list(q, list, true);
+  P.scalars = acc_scalars;
+  if (rc != SG_OK) return rc;
+  const uint64_t* scal = q->h_acc.data();
+  if (scal[2] != 0) {
+    c->set_err("query: rows fall outside the planned time axis (time_min/time_max too narrow)");
+    return SG_ERR_INVALID;
+  }
+  if (scal[4] != 0) {
+    c->set_err("query: the hashed slot space filled up (more distinct group keys than its table holds)");
+    return SG_ERR_UNSUPPORTED;
+  }
+  uint32_t* const d_ids = q->d_hids;
+  uint32_t* const d_id2key = q->d_hids + q->hcap;
+  unsigned int* const d_live = reinterpret_cast<unsigned int*>(q->d_disc + SCALAR_WORDS);
+  cudaEvent_t e0 = q->ev0, e1 = q->ev1;
+  CUDA_TRY(c, cudaEventRecord(e0, c->stream));
+  const unsigned grid = (unsigned)std::min<uint64_t>(((uint64_t)q->hcap + 255) / 256, (uint64_t)std::max(c->sm_count, 1) * 8);
+  assign_ids<<<grid, 256, 0, c->stream>>>(q->d_hkeys, q->hcap, d_ids, d_id2key, d_live);
+  CUDA_TRY(c, cudaGetLastError());
+  CUDA_TRY(c, cudaEventRecord(e1, c->stream));
+  uint64_t live = 0;
+  CUDA_TRY(c, cudaMemcpyAsync(&live, q->d_disc + SCALAR_WORDS, 8, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+  q->d2h_bytes += 8;
+  q->launches += 1;
+  float ids_ms = 0;
+  CUDA_TRY(c, cudaEventElapsedTime(&ids_ms, e0, e1));
+  q->kernel_ms += ids_ms;
+  uint64_t budget = ACC_LIMIT_BYTES;
+  if (const char* e = getenv("SG_SPARSE_BUDGET_MIB")) budget = (uint64_t)std::max(atoll(e), 0ll) << 20;
+  if (getenv("SG_PLAN_TRACE"))
+    fprintf(stderr, "sg_sparse: live=%llu table=%u discover_ms=%.4f ids_ms=%.4f\n", (unsigned long long)live, q->hcap,
+            q->disc_ms, (double)ids_ms);
+  if (sum_region_bytes(q, live) > budget) {
+    c->set_err("query: sparse group accumulators for " + std::to_string(live) + " live groups exceed " +
+               std::to_string(budget >> 20) + " MiB");
+    return SG_ERR_UNSUPPORTED;
+  }
+  // accumulators for the live groups (a run over a table with more live groups needs a larger array)
+  P.nslots = (uint32_t)live;
+  rc = layout_accumulators(q, P.nslots);
+  if (rc != SG_OK) return rc;
+  pool_release(c, q->d_acc);
+  q->d_acc = nullptr;
+  CUDA_TRY(c, pool_alloc(c, (void**)&q->d_acc, q->acc_words * 8));
+  point_plan(q);
   return SG_OK;
 }
 
@@ -3137,8 +3284,10 @@ int build_result(sg_query* q, sg_result** out) {
       c->set_err("query: StrReplace / weights over a hashed slot space are not in this build");
       return SG_ERR_UNSUPPORTED;
     }
+    // slot -> key: the table itself, or for a sparse plan its id -> key array (L entries, nothing sized by the table)
     q->h_hkeys.resize(P.nslots);
-    CUDA_TRY(c, cudaMemcpyAsync(q->h_hkeys.data(), q->d_hkeys, (size_t)P.nslots * 4, cudaMemcpyDeviceToHost, c->stream));
+    const uint32_t* keys = q->sparse ? q->d_hids + q->hcap : q->d_hkeys;
+    if (P.nslots) CUDA_TRY(c, cudaMemcpyAsync(q->h_hkeys.data(), keys, (size_t)P.nslots * 4, cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     q->d2h_bytes += (int64_t)P.nslots * 4;
   }
@@ -3467,6 +3616,17 @@ int sg_query_set_str_replace(sg_query* q, int32_t col, const char* bytes, const 
   return SG_OK;
 }
 
+int sg_query_set_sparse_groups(sg_query* q, int32_t on) {
+  if (!q) return SG_ERR_INVALID;
+  if (on != 0 && on != 1) {
+    q->ctx->set_err("sg_query_set_sparse_groups: on must be 0 or 1");
+    return SG_ERR_INVALID;
+  }
+  if (on != q->sparse_req) q->planned = false;  // the next sg_query_run plans again
+  q->sparse_req = on;
+  return SG_OK;
+}
+
 int sg_query_should_load(sg_query* q, const sg_block_desc* b) {
   if (!q || !b) return SG_ERR_INVALID;
   std::vector<sg_int_info> info(b->info, b->info + b->ninfo);
@@ -3565,6 +3725,10 @@ int sg_query_run(sg_query* q) {
   // a block found broken by the kernel ("BLOCK SIZE CHANGED", row id >= NumRecords)
   // must contribute nothing: rerun without it (rare path)
   for (int attempt = 0; attempt < 8; attempt++) {
+    if (q->sparse) {  // (every attempt rediscovers: the keys of a dropped block get no id)
+      rc = discover_groups(q, list);
+      if (rc != SG_OK) return rc;
+    }
     rc = reset_accumulators(q);
     if (rc != SG_OK) return rc;
     rc = run_list(q, list);
@@ -3573,6 +3737,10 @@ int sg_query_run(sg_query* q) {
     if (scal[2] != 0) {
       c->set_err("query: rows fall outside the planned time axis (time_min/time_max too narrow)");
       return SG_ERR_INVALID;
+    }
+    if (q->sparse && scal[5] != 0) {
+      c->set_err("query: " + std::to_string(scal[5]) + " rows' group keys were missing from the discovered sparse groups");
+      return SG_ERR_STATE;
     }
     if (scal[1] == 0) break;
     std::vector<uint32_t> status(t->blocks.size());
@@ -3604,6 +3772,11 @@ int sg_query_submit_block(sg_query* q, const sg_block_desc* b) {
   // streaming path: the block is staged into the query's table (H2D on the copy
   // stream) and scanned by sg_query_finish; zone-map pruning happens before staging
   if (!q || !b) return SG_ERR_INVALID;
+  if (q->sparse_req) {
+    q->ctx->set_err("sg_query_submit_block: sparse group accumulators scan every block twice (discovery, then "
+                    "aggregation); stage the blocks with sg_table_add_block(s) and use sg_query_run");
+    return SG_ERR_UNSUPPORTED;
+  }
   std::vector<sg_int_info> info(b->info, b->info + b->ninfo);
   if (!should_load(q, info)) {
     q->stream_skipped++;

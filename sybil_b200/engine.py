@@ -40,6 +40,10 @@ class _Flags:
         # previous row that has it, as LoadAndQueryRecords does (sg_query_desc.weight_carry).  False: a weighted
         # query over such rows fails with SG_ERR_UNSUPPORTED.
         self.WEIGHT_CARRY = False
+        # The engine's own flag: a group-by whose accumulators would pass 24 GiB holds accumulators for the groups
+        # that occur only, as sybil's result map does (sg_query_set_sparse_groups).  False: such a query fails
+        # with SG_ERR_UNSUPPORTED.
+        self.SPARSE_GROUPS = False
 
 
 FLAGS = _Flags()
@@ -515,6 +519,8 @@ class PreparedQuery:
         if not self.q:
             raise SybilGpuError(F.SG_ERR_INVALID, ctx.err())
         try:
+            if FLAGS.SPARSE_GROUPS:
+                ctx.check(lib.sg_query_set_sparse_groups(self.q, 1))
             for name, strs in rewritten.items():
                 blob = b"".join(strs)
                 offs = np.zeros(len(strs) + 1, np.uint32)
