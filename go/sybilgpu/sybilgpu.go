@@ -244,6 +244,9 @@ type Query struct {
 	// A group-by whose accumulators would pass 24 GiB keeps accumulators for the groups that occur only, as sybil's
 	// result map does (sg_query_set_sparse_groups).  False: such a query fails with SG_ERR_UNSUPPORTED.
 	SparseGroups bool
+	// Weighted and StrReplace group-bys whose keys go through the device hash table (or sparse group accumulators)
+	// are folded on the device (sg_query_set_hashed_folds).  False: such a query fails with SG_ERR_UNSUPPORTED.
+	HashedFolds bool
 }
 
 // StrReplaced carries, for one str column, the rewritten text of every string of its global dictionary
@@ -332,6 +335,9 @@ func (t *Table) Run(q *Query, allreduce bool) (*C.sg_result, error) {
 	}
 	defer C.sg_query_free(h)
 	if q.SparseGroups && C.sg_query_set_sparse_groups(h, 1) != C.SG_OK {
+		return nil, t.c.err()
+	}
+	if q.HashedFolds && C.sg_query_set_hashed_folds(h, 1) != C.SG_OK {
 		return nil, t.c.err()
 	}
 	for i, f := range q.Filters {

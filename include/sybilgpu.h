@@ -35,7 +35,8 @@ extern "C" {
  * a hash table on the device keyed by the combined code (single GPU; at most 2^25 distinct groups per query).
  * Accumulators (count, sums, histogram counters per slot of that array or table) may take up to 24 GiB; with
  * sg_query_set_sparse_groups(q, 1) a plan past that holds accumulators for the groups that occur only, and the
- * 24 GiB limit applies to those (single GPU, sg_query_run only, no weights or StrReplace). */
+ * 24 GiB limit applies to those (single GPU, sg_query_run only).  Weights and StrReplace over the hash table, or
+ * over sparse accumulators, need sg_query_set_hashed_folds(q, 1). */
 #define SG_MAX_FILTERS 15
 #define SG_MAX_GROUPS 8
 #define SG_MAX_AGGS 16
@@ -298,11 +299,23 @@ int sg_query_set_str_replace(sg_query* q, int32_t col_slot, const char* bytes, c
  *   1 = such a plan scans twice: a discovery pass collects the group keys of every row that passes into a table on
  *       the device and numbers them, then the aggregation pass accumulates into arrays sized by those L live
  *       groups, and only those are read back.  It fails with SG_ERR_UNSUPPORTED when the L groups' accumulators
- *       pass 24 GiB, for weighted queries and StrReplace, and under sg_query_allreduce.  Plans within the limit
- *       run as with 0.  The streaming path needs every block staged before the first pass: sg_query_submit_block
- *       fails with SG_ERR_UNSUPPORTED while the setting is 1.
+ *       pass 24 GiB, for weighted queries and StrReplace unless sg_query_set_hashed_folds(q, 1), and under
+ *       sg_query_allreduce.  Plans within the limit run as with 0.  The streaming path needs every block staged
+ *       before the first pass: sg_query_submit_block fails with SG_ERR_UNSUPPORTED while the setting is 1.
  * Any other value is SG_ERR_INVALID.  Takes effect at the next sg_query_run (a prepared query plans again). */
 int sg_query_set_sparse_groups(sg_query* q, int32_t on);
+/* Weights and StrReplace over hashed group keys (the Go reference's result map holds the keys that occur, and every
+ * row adds its weight, aggregate.go:100-102,186-203).  A weighted query groups by the weight value as a hidden axis,
+ * and StrReplace groups by the original strings; both are then folded: every (group, weight value, original string)
+ * entry's accumulators are combined onto the group it belongs to, multiplied by its weight.
+ *   0 (default) = a weighted or StrReplace query whose group keys go through the hashed table (past 2^26 codes) fails
+ *       with SG_ERR_UNSUPPORTED after the scan, and with sparse group accumulators it is refused when planned;
+ *   1 = such a query is folded on the device, behind the scan and before anything is read back, on hashed plans and,
+ *       with sg_query_set_sparse_groups(q, 1), on sparse ones (single GPU).  Rows without the weight column still
+ *       need weight_carry; a table the folded keys fill up still fails with SG_ERR_UNSUPPORTED.
+ * Dense plans fold on the host with either value.  Any other value is SG_ERR_INVALID.  Takes effect at the next
+ * sg_query_run (a prepared query plans again). */
+int sg_query_set_hashed_folds(sg_query* q, int32_t on);
 /* ShouldLoadBlockFromDir (table_block_io.go:110-182): 1 = load, 0 = pruned */
 int sg_query_should_load(sg_query* q, const sg_block_desc* block);
 /* Resident path: run the scan over every staged block of the table

@@ -118,6 +118,7 @@ SYMBOLS = {
     "sg_query_set_str_lut": (C.c_int, [P, C.c_int32, P, C.c_int64]),
     "sg_query_set_str_replace": (C.c_int, [P, C.c_int32, P, P, C.c_int64]),
     "sg_query_set_sparse_groups": (C.c_int, [P, C.c_int32]),
+    "sg_query_set_hashed_folds": (C.c_int, [P, C.c_int32]),
     "sg_query_should_load": (C.c_int, [P, C.POINTER(sg_block_desc)]),
     "sg_query_run": (C.c_int, [P]),
     "sg_query_submit_block": (C.c_int, [P, C.POINTER(sg_block_desc)]),

@@ -1307,6 +1307,20 @@ struct GroupDim {  // one axis of the dense slot space
   uint32_t radix = 1, stride = 1;
 };
 
+// The canonical key of a table entry (device folds, sg_query_set_hashed_folds): the entry's code with the weight
+// digit set to 0 and each rewritten axis' digit replaced by its class representative's (0 when the string rewrites
+// to "": the missing group, DESIGN.md §7); every other digit, time included, unchanged.  What fold_axes does per
+// dense slot, restated per key.
+struct FoldKey {
+  uint32_t naxes = 0;  // rewritten (StrReplace) axes
+  uint32_t stride[SG_MAX_GROUPS] = {}, radix[SG_MAX_GROUPS] = {};
+  uint32_t lut[SG_MAX_GROUPS] = {};  // offset of the axis' table in luts
+  uint32_t wstride = 0, wradix = 0;  // the weight axis (wradix 0: unweighted)
+  uint32_t wcarry = 0;
+  const int64_t* wmul = nullptr;     // per weight code its multiplier (code 0: weight 1 under wcarry)
+  const uint32_t* luts = nullptr;    // per rewritten axis, radix entries: digit -> canonical digit
+};
+
 struct ResultGroup {
   std::vector<uint64_t> key;
   std::string skey;
@@ -1433,8 +1447,18 @@ struct sg_query {
   int32_t sparse_req = 0;        // the setter's value, applied by the next plan
   bool sparse = false;           // this plan takes the path
   uint32_t* d_hids = nullptr;    // [hcap] table entry -> dense id, then [hcap] dense id -> key (code + 1)
-  uint64_t* d_disc = nullptr;    // the discovery launch's scalars (SCALAR_WORDS), then the live group count
+  uint64_t* d_disc = nullptr;    // the discovery launch's scalars (SCALAR_WORDS), then the live and canonical counts
   double disc_ms = 0;            // the last discovery launch (SG_PLAN_TRACE)
+  // device folds (sg_query_set_hashed_folds): a hashed or sparse plan with weights or StrReplace combines the
+  // accumulators of every table entry onto its canonical entry on the device (fold_insert, fold_rows)
+  int32_t hfold_req = 0;           // the setter's value, applied by the next plan
+  bool dfold = false;              // this plan folds on the device
+  FoldKey fkey;                    // its device pointers name d_fold
+  void* d_fold = nullptr;          // the weight multipliers (int64 per weight code), then the rewrite tables (uint32)
+  uint64_t* d_samples = nullptr;   // [n] rows per accumulator row after the fold, then [n] each row's own rows
+  uint32_t canon_live = 0;         // sparse: canonical entries, which hold ids 0..canon_live-1
+  double insert_ms = 0, fold_ms = 0;
+  cudaEvent_t ev2 = nullptr, ev3 = nullptr;
   // accumulators as read back right behind the kernel (small plans): spares build_result a blocking copy
   std::vector<uint64_t> h_acc;
   bool h_acc_valid = false;
@@ -1481,6 +1505,10 @@ void free_device(sg_query* q) {
   q->d_hids = nullptr;
   pool_release(c, q->d_disc);
   q->d_disc = nullptr;
+  pool_release(c, q->d_fold);
+  q->d_fold = nullptr;
+  pool_release(c, q->d_samples);
+  q->d_samples = nullptr;
   pool_release(c, q->d_gbinpay);
   pool_release(c, q->d_gdummy);
   for (auto p : q->d_luts) pool_release(c, p);
@@ -1926,13 +1954,16 @@ int make_plan(sg_query* q, const std::vector<uint32_t>& list) {
   q->sparse = q->sparse_req == 1 &&
               (getenv("SG_FORCE_SPARSE_GROUPS") || sum_region_bytes(q, hashed ? cap : stride) > ACC_LIMIT_BYTES);
   if (q->sparse) {
-    if (weighted || !q->repl.empty()) {
+    if ((weighted || !q->repl.empty()) && q->hfold_req != 1) {
       c->set_err("query: weights / StrReplace are not combined with sparse group accumulators in this build");
       return SG_ERR_UNSUPPORTED;
     }
     hashed = true;
   }
   q->hashed = hashed;
+  // ---- device folds (sg_query_set_hashed_folds): a hashed slot space has no slot arithmetic for fold_axes, so its
+  // weight axis and rewritten strings are folded over the table's entries on the device (fold_insert, fold_rows)
+  q->dfold = hashed && q->hfold_req == 1 && (weighted || !q->repl.empty());
   if (stride > (uint64_t)MAX_SLOTS && !q->hashed) {
     c->set_err("query: group-by cardinality product exceeds the dense slot space");
     return SG_ERR_UNSUPPORTED;
@@ -2251,6 +2282,7 @@ int make_plan(sg_query* q, const std::vector<uint32_t>& list) {
 }
 
 void point_plan(sg_query* q);
+int upload_fold(sg_query* q);
 
 int alloc_device(sg_query* q) {
   sg_ctx* c = q->ctx;
@@ -2285,13 +2317,77 @@ int alloc_device(sg_query* q) {
   if (q->hashed) CUDA_TRY(c, pool_alloc(c, (void**)&q->d_hkeys, (size_t)q->hcap * 4));
   if (q->sparse) {
     CUDA_TRY(c, pool_alloc(c, (void**)&q->d_hids, (size_t)q->hcap * 8));
-    if (!q->d_disc) CUDA_TRY(c, pool_alloc(c, (void**)&q->d_disc, (SCALAR_WORDS + 1) * 8));
+    if (!q->d_disc) CUDA_TRY(c, pool_alloc(c, (void**)&q->d_disc, (SCALAR_WORDS + 2) * 8));
   }
   if (!q->ev0) {
     CUDA_TRY(c, cudaEventCreate(&q->ev0));
     CUDA_TRY(c, cudaEventCreate(&q->ev1));
   }
+  pool_release(c, q->d_samples);
+  q->d_samples = nullptr;
+  if (q->dfold) {
+    int rc = upload_fold(q);
+    if (rc != SG_OK) return rc;
+    // (a sparse plan's rows are counted by its discovery launch: discover_groups allocates them)
+    if (!q->sparse) CUDA_TRY(c, pool_alloc(c, (void**)&q->d_samples, (size_t)q->hcap * 16));
+    if (!q->ev2) {
+      CUDA_TRY(c, cudaEventCreate(&q->ev2));
+      CUDA_TRY(c, cudaEventCreate(&q->ev3));
+    }
+  }
   point_plan(q);
+  return SG_OK;
+}
+
+// The device fold's tables (FoldKey): the weight axis' multipliers and each rewritten axis' digit -> canonical digit
+// map, from the same dictionaries and StrReplace classes fold_axes reads
+int upload_fold(sg_query* q) {
+  sg_ctx* c = q->ctx;
+  FoldKey& F = q->fkey;
+  F = FoldKey();
+  F.wcarry = q->plan.wcarry;
+  std::vector<int64_t> wmul;
+  std::vector<uint32_t> luts;
+  for (const GroupDim& d : q->dims) {
+    if (d.is_weight) {
+      const std::vector<int64_t>& vals = q->table->idict[(size_t)d.col].vals;
+      if (vals.size() + 1 != (size_t)d.radix) {
+        c->set_err("query: the weight column's value dictionary changed under the query");
+        return SG_ERR_STATE;
+      }
+      F.wstride = d.stride;
+      F.wradix = d.radix;
+      wmul.push_back(1);
+      wmul.insert(wmul.end(), vals.begin(), vals.end());
+    } else if (d.is_str && q->repl.count(d.col)) {
+      const auto& R = q->repl.at(d.col);
+      if (R.canon.size() + 1 != (size_t)d.radix || R.strs.size() != R.canon.size()) {
+        c->set_err("query: the dictionary of a StrReplace column grew after sg_query_set_str_replace");
+        return SG_ERR_STATE;
+      }
+      F.stride[F.naxes] = d.stride;
+      F.radix[F.naxes] = d.radix;
+      F.lut[F.naxes] = (uint32_t)luts.size();
+      F.naxes++;
+      luts.push_back(0);
+      for (size_t i = 0; i < R.canon.size(); i++) luts.push_back(R.strs[i].empty() ? 0u : R.canon[i] + 1u);
+    }
+  }
+  const size_t wbytes = wmul.size() * 8, bytes = wbytes + luts.size() * 4;
+  pool_release(c, q->d_fold);
+  q->d_fold = nullptr;
+  CUDA_TRY(c, pool_alloc(c, &q->d_fold, std::max<size_t>(bytes, 8)));
+  char* hp = c->scratch(std::max<size_t>(bytes, 8));
+  if (!hp) {
+    c->set_err("cudaHostAlloc (query scratch) failed");
+    return SG_ERR_CUDA;
+  }
+  memcpy(hp, wmul.data(), wbytes);
+  memcpy(hp + wbytes, luts.data(), luts.size() * 4);
+  CUDA_TRY(c, cudaMemcpyAsync(q->d_fold, hp, bytes, cudaMemcpyHostToDevice, c->stream));
+  CUDA_TRY(c, cudaStreamSynchronize(c->stream));  // (the scratch is reused by the next launch)
+  F.wmul = wmul.empty() ? nullptr : (const int64_t*)q->d_fold;
+  F.luts = luts.empty() ? nullptr : (const uint32_t*)((char*)q->d_fold + wbytes);
   return SG_OK;
 }
 
@@ -2430,6 +2526,8 @@ int reset_accumulators(sg_query* q) {
   return SG_OK;
 }
 
+int device_fold(sg_query* q, bool discover);
+
 // one launch of the scan kernel over `list`.  discover: the discovery launch of a sparse plan (its scalars go to
 // d_disc and are what comes back)
 int run_list(sg_query* q, const std::vector<uint32_t>& list, bool discover = false) {
@@ -2463,7 +2561,9 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list, bool discover = fal
   // small accumulator arrays come back right behind the scan (build_result then needs no further copy) — unless a
   // cross-GPU merge follows, which reads the MERGED array back itself: then only the scalars (broken blocks) do
   const bool merge_follows = c->comm != nullptr && c->nranks > 1;
-  const size_t acc_back = (!discover && !merge_follows && q->acc_words * 8 <= ((size_t)4 << 20)) ? q->acc_words * 8 : 64;
+  // (a folded sparse plan: build_result reads the canonical groups' rows alone)
+  const bool whole_back = !discover && !merge_follows && !(q->sparse && q->dfold);
+  const size_t acc_back = (whole_back && q->acc_words * 8 <= ((size_t)4 << 20)) ? q->acc_words * 8 : 64;
   const size_t off_items = (sizeof(Plan) + 255) & ~(size_t)255;
   const size_t off_acc = off_items + ((items.size() * 16 + 255) & ~(size_t)255);
   char* hp = c->scratch(off_acc + acc_back);
@@ -2615,6 +2715,7 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list, bool discover = fal
       fprintf(stderr, " agg%d=[fmin=%lld fmax=%lld hist32=%d nocarry=%d]", a, fmin, fmax, hist32 ? 1 : 0, nocarry ? 1 : 0);
     }
     if (q->sparse) fprintf(stderr, " sparse=1 live=%u table=%u", P.nslots, q->hcap);
+    if (q->dfold) fprintf(stderr, " fold=1");
     fprintf(stderr, "\n");
   }
   int grid = (int)std::min<size_t>((size_t)q->grid, std::max<size_t>(items.size(), 1));
@@ -2625,6 +2726,10 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list, bool discover = fal
     return SG_ERR_CUDA;
   }
   CUDA_TRY(c, cudaEventRecord(q->ev1, c->stream));
+  if (q->dfold) {  // after the last scan of the run and before anything is read back
+    rc = device_fold(q, discover);
+    if (rc != SG_OK) return rc;
+  }
   const bool to_pin = acc_back == q->acc_words * 8 && acc_back >= ((size_t)32 << 10);
   q->h_pin_valid = false;
   if (to_pin) {
@@ -2651,6 +2756,18 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list, bool discover = fal
   q->kernel_ms += ms;
   if (discover) q->disc_ms = ms;
   q->launches += 1;
+  if (q->dfold) {
+    float ims = 0, fms = 0;
+    CUDA_TRY(c, cudaEventElapsedTime(&ims, q->ev1, q->ev2));
+    CUDA_TRY(c, cudaEventElapsedTime(&fms, q->ev2, q->ev3));
+    q->kernel_ms += ims + fms;
+    if (discover || !q->sparse) q->insert_ms = ims;
+    q->fold_ms = fms;
+    // scalars [6] / [7]: the table's occupied entries / the canonical ones among them (fold_rows)
+    if (!discover && getenv("SG_PLAN_TRACE"))
+      fprintf(stderr, "sg_fold: entries=%llu canon=%llu insert_ms=%.4f fold_ms=%.4f\n", (unsigned long long)q->h_acc[6],
+              (unsigned long long)q->h_acc[7], q->insert_ms, q->fold_ms);
+  }
   if (d_dbg) {
     std::vector<unsigned long long> hd((size_t)q->grid * 16);
     cudaMemcpy(hd.data(), d_dbg, hd.size() * 8, cudaMemcpyDeviceToHost);
@@ -2674,15 +2791,29 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list, bool discover = fal
   return SG_OK;
 }
 
+__device__ __forceinline__ uint32_t canon_code(const FoldKey& F, uint32_t code) {
+  uint32_t out = code;
+#pragma unroll
+  for (uint32_t a = 0; a < SG_MAX_GROUPS; a++) {  // (unrolled: the parameter arrays stay out of local memory)
+    if (a >= F.naxes) break;
+    const uint32_t d = (code / F.stride[a]) % F.radix[a];
+    out += (F.luts[F.lut[a] + d] - d) * F.stride[a];  // (mod 2^32: the result is a code again)
+  }
+  if (F.wradix) out -= ((code / F.wstride) % F.wradix) * F.wstride;
+  return out;
+}
+
 // Dense ids of the sparse path: every occupied entry of the table gets an id in 0..L-1 (in no set order: the result
 // orders its groups itself), id2key[id] = the entry's key (code + 1), *live = L.  One warp-aggregated atomic per warp
-// and step; the launch runs after every insert of the discovery launch is done.
+// and step; the launch runs after every insert of the discovery launch is done.  pick (device folds): 1 numbers the
+// canonical entries only, 2 the others, continuing from *live; 0 every entry.
 __global__ void assign_ids(const uint32_t* __restrict__ keys, uint32_t cap, uint32_t* __restrict__ ids,
-                           uint32_t* __restrict__ id2key, unsigned int* live) {
+                           uint32_t* __restrict__ id2key, unsigned int* live, FoldKey F, int pick) {
   const uint32_t stride = gridDim.x * blockDim.x;
   for (uint32_t base = blockIdx.x * blockDim.x; base < cap; base += stride) {
     const uint32_t i = base + threadIdx.x;
-    const uint32_t k = i < cap ? keys[i] : 0u;
+    uint32_t k = i < cap ? keys[i] : 0u;
+    if (k != 0u && pick != 0 && (canon_code(F, k - 1u) == k - 1u) != (pick == 1)) k = 0u;
     const unsigned m = __ballot_sync(0xffffffffu, k != 0u);
     if (!m) continue;
     const int lane = (int)(threadIdx.x & 31u);
@@ -2697,6 +2828,179 @@ __global__ void assign_ids(const uint32_t* __restrict__ keys, uint32_t cap, uint
   }
 }
 
+// ---- device folds (sg_query_set_hashed_folds) ------------------------------------------------------------------
+// Canonical insert: every occupied entry whose key is not canonical inserts its canonical key into the same table,
+// with the scan's probing (a hashed plan: after the scan; a sparse plan: after discovery, so that the canonical
+// entries get ids and accumulator rows).  An entry read while another thread inserts it is canonical: nothing to
+// do.  scalars[4] counts inserts that found the table full, as the scan does.
+__global__ void fold_insert(uint32_t* hk, uint32_t hmask, FoldKey F, unsigned long long* scalars) {
+  const uint32_t stride = gridDim.x * blockDim.x;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i <= hmask; i += stride) {
+    const uint32_t k = hk[i];
+    if (k == 0u) continue;
+    const uint32_t key = canon_code(F, k - 1u) + 1u;
+    if (key == k) continue;
+    uint32_t idx = slot_hash(key) & hmask, probes = 0;
+    for (;;) {
+      const uint32_t old = atomicCAS(hk + idx, 0u, key);
+      if (old == 0u || old == key) break;
+      idx = (idx + 1u) & hmask;
+      if (++probes > hmask) {
+        atomicAdd(scalars + 4, 1ull);
+        break;
+      }
+    }
+  }
+}
+
+// the accumulator regions a fold combines, as offsets into the accumulator array
+struct FoldAcc {
+  uint64_t* acc;
+  const uint32_t* hk;
+  uint32_t hmask;
+  const uint32_t* ids;         // sparse plans: table entry -> accumulator row; nullptr: the entry itself
+  const unsigned long long* own;  // each row's own rows (the count array as the scan left it)
+  unsigned long long* samples;    // rows per row after the fold (zeroed)
+  unsigned long long* scalars;
+  uint32_t nadd, nmax, nbk;
+  size_t add_off[1 + 2 * SG_MAX_AGGS];  // one word per row, added: count, exact sums, hist Counts
+  size_t max_off[SG_MAX_AGGS];          // one word per row, max: the MAX region
+  size_t bk_off[SG_MAX_AGGS];           // bk_nv words per row, added: bucket counters
+  uint32_t bk_nv[SG_MAX_AGGS];
+};
+
+// Fold: every non-canonical entry e with canonical entry c and weight multiplier w adds acc[e] * w into acc[c]
+// (uint64, wrapping: fold_axes' arithmetic) and takes the max into the MAX region unmultiplied, then clears e; its
+// rows go to samples[c], where a canonical entry's own rows also land.  Integer sums in any order: the result is
+// the dense path's bit for bit.  Each warp reads 32 entries, then folds its sources one after the other with the
+// lanes striding over the source's words.  scalars: [3] rows on weight code 0 without carry (refused), [6] occupied
+// entries, [7] canonical ones.
+__global__ void fold_rows(FoldAcc A, FoldKey F) {
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
+  constexpr uint32_t NONE = 0xffffffffu;
+  for (uint32_t base = warp * 32u; base <= A.hmask; base += nwarps * 32u) {
+    const uint32_t i = base + lane;
+    const uint32_t k = i <= A.hmask ? A.hk[i] : 0u;
+    uint32_t src = NONE, dst = 0u;
+    unsigned long long mul = 1ull;
+    bool canon = false;
+    if (k != 0u) {
+      const uint32_t code = k - 1u, cc = canon_code(F, code);
+      const uint32_t row = A.ids ? A.ids[i] : i;
+      const unsigned long long own = A.own[row];
+      uint32_t to = row;
+      if (F.wradix) {
+        const uint32_t wd = (code / F.wstride) % F.wradix;
+        if (wd == 0u && !F.wcarry && own) atomicAdd(A.scalars + 3, own);
+        mul = (unsigned long long)F.wmul[wd];
+      }
+      canon = cc == code;
+      if (!canon) {
+        uint32_t j = slot_hash(cc + 1u) & A.hmask;
+        for (uint32_t probes = 0;; probes++) {
+          const uint32_t kk = A.hk[j];
+          if (kk == cc + 1u) break;
+          if (kk == 0u || probes >= A.hmask) {  // (only after the insert found the table full: refused)
+            j = NONE;
+            break;
+          }
+          j = (j + 1u) & A.hmask;
+        }
+        if (j != NONE) {
+          to = A.ids ? A.ids[j] : j;
+          src = row;
+          dst = to;
+        }
+      }
+      if (own) atomicAdd(A.samples + to, own);
+    }
+    const unsigned occ = __ballot_sync(0xffffffffu, k != 0u), can = __ballot_sync(0xffffffffu, canon);
+    if (lane == 0 && occ) {
+      atomicAdd(A.scalars + 6, (unsigned long long)__popc(occ));
+      if (can) atomicAdd(A.scalars + 7, (unsigned long long)__popc(can));
+    }
+    for (unsigned m = __ballot_sync(0xffffffffu, src != NONE); m; m &= m - 1u) {
+      const int l = __ffs((int)m) - 1;
+      const uint32_t s = __shfl_sync(0xffffffffu, src, l), d = __shfl_sync(0xffffffffu, dst, l);
+      const unsigned long long w = __shfl_sync(0xffffffffu, mul, l);
+      for (uint32_t r = lane; r < A.nadd; r += 32u) {
+        unsigned long long* p = (unsigned long long*)A.acc + A.add_off[r];
+        const unsigned long long v = p[s];
+        if (v) {
+          atomicAdd(p + d, v * w);
+          p[s] = 0ull;
+        }
+      }
+      for (uint32_t r = lane; r < A.nmax; r += 32u) {
+        long long* p = (long long*)A.acc + A.max_off[r];
+        const long long v = p[s];
+        if (v != INT64_MIN) {
+          atomicMax(p + d, v);
+          p[s] = INT64_MIN;
+        }
+      }
+      for (uint32_t b = 0; b < A.nbk; b++) {
+        const size_t nv = A.bk_nv[b];
+        unsigned long long* p = (unsigned long long*)A.acc + A.bk_off[b];
+        for (size_t x = lane; x < nv; x += 32u) {
+          const unsigned long long v = p[(size_t)s * nv + x];
+          if (v) {
+            atomicAdd(p + (size_t)d * nv + x, v * w);
+            p[(size_t)s * nv + x] = 0ull;
+          }
+        }
+      }
+    }
+  }
+}
+
+// The device fold of a run, queued behind its scan launch: the canonical insert (a hashed plan, or a sparse plan's
+// discovery launch), then the fold (every launch that aggregates).  ev1 -> ev2 times the insert, ev2 -> ev3 the fold.
+int device_fold(sg_query* q, bool discover) {
+  sg_ctx* c = q->ctx;
+  const Plan& P = q->plan;
+  const uint32_t cap = q->hcap;
+  const unsigned grid = (unsigned)std::min<uint64_t>(((uint64_t)cap + 255) / 256, (uint64_t)std::max(c->sm_count, 1) * 8);
+  unsigned long long* const scalars = (unsigned long long*)(discover ? q->d_disc : q->d_acc);
+  if (discover || !q->sparse) {
+    fold_insert<<<grid, 256, 0, c->stream>>>(q->d_hkeys, cap - 1u, q->fkey, scalars);
+    CUDA_TRY(c, cudaGetLastError());
+    q->launches += 1;
+  }
+  CUDA_TRY(c, cudaEventRecord(q->ev2, c->stream));
+  if (!discover) {
+    const size_t n = P.nslots;  // accumulator rows: the table's entries, or a sparse plan's live groups
+    FoldAcc A;
+    memset(&A, 0, sizeof(A));
+    A.acc = q->d_acc;
+    A.hk = q->d_hkeys;
+    A.hmask = cap - 1u;
+    A.ids = q->sparse ? q->d_hids : nullptr;
+    A.samples = (unsigned long long*)q->d_samples;
+    A.own = (const unsigned long long*)(q->d_samples + n);
+    A.scalars = scalars;
+    A.add_off[A.nadd++] = q->off_count;
+    for (int a = 0; a < P.naggs; a++) {
+      A.add_off[A.nadd++] = q->off_sum[(size_t)a];
+      A.add_off[A.nadd++] = q->off_hcount[(size_t)a];
+      A.max_off[A.nmax++] = q->off_vmax[(size_t)a];
+      const uint32_t nv = q->layouts[(size_t)a].nvals_total;
+      if (nv) {
+        A.bk_off[A.nbk] = q->off_buckets[(size_t)a];
+        A.bk_nv[A.nbk++] = nv;
+      }
+    }
+    CUDA_TRY(c, cudaMemsetAsync(q->d_samples, 0, n * 8, c->stream));
+    CUDA_TRY(c, cudaMemcpyAsync(q->d_samples + n, q->d_acc + q->off_count, n * 8, cudaMemcpyDeviceToDevice, c->stream));
+    fold_rows<<<grid, 256, 0, c->stream>>>(A, q->fkey);
+    CUDA_TRY(c, cudaGetLastError());
+    q->launches += 1;
+  }
+  CUDA_TRY(c, cudaEventRecord(q->ev3, c->stream));
+  return SG_OK;
+}
+
 // Sparse group accumulators, before the aggregation launch: the discovery launch fills the table with the code of
 // every row that passes, assign_ids numbers the entries, and the accumulators are laid out for the L live groups.
 // Refuses when L groups' accumulators pass 24 GiB (tests: SG_SPARSE_BUDGET_MIB=n lowers that budget); the query's
@@ -2705,7 +3009,7 @@ int discover_groups(sg_query* q, const std::vector<uint32_t>& list) {
   sg_ctx* c = q->ctx;
   Plan& P = q->plan;
   CUDA_TRY(c, cudaMemsetAsync(q->d_hkeys, 0, (size_t)q->hcap * 4, c->stream));
-  CUDA_TRY(c, cudaMemsetAsync(q->d_disc, 0, (SCALAR_WORDS + 1) * 8, c->stream));
+  CUDA_TRY(c, cudaMemsetAsync(q->d_disc, 0, (SCALAR_WORDS + 2) * 8, c->stream));
   uint64_t* const acc_scalars = P.scalars;
   P.scalars = q->d_disc;
   int rc = run_list(q, list, true);
@@ -2726,14 +3030,22 @@ int discover_groups(sg_query* q, const std::vector<uint32_t>& list) {
   cudaEvent_t e0 = q->ev0, e1 = q->ev1;
   CUDA_TRY(c, cudaEventRecord(e0, c->stream));
   const unsigned grid = (unsigned)std::min<uint64_t>(((uint64_t)q->hcap + 255) / 256, (uint64_t)std::max(c->sm_count, 1) * 8);
-  assign_ids<<<grid, 256, 0, c->stream>>>(q->d_hkeys, q->hcap, d_ids, d_id2key, d_live);
-  CUDA_TRY(c, cudaGetLastError());
+  // a folded plan numbers its canonical entries first (ids 0..L'-1: the rows its result reads back), then the others
+  const int npass = q->dfold ? 2 : 1;
+  for (int pass = 0; pass < npass; pass++) {
+    assign_ids<<<grid, 256, 0, c->stream>>>(q->d_hkeys, q->hcap, d_ids, d_id2key, d_live, q->fkey, q->dfold ? pass + 1 : 0);
+    CUDA_TRY(c, cudaGetLastError());
+    if (q->dfold && pass == 0)
+      CUDA_TRY(c, cudaMemcpyAsync(q->d_disc + SCALAR_WORDS + 1, q->d_disc + SCALAR_WORDS, 8, cudaMemcpyDeviceToDevice, c->stream));
+  }
   CUDA_TRY(c, cudaEventRecord(e1, c->stream));
-  uint64_t live = 0;
-  CUDA_TRY(c, cudaMemcpyAsync(&live, q->d_disc + SCALAR_WORDS, 8, cudaMemcpyDeviceToHost, c->stream));
+  uint64_t counts[2] = {0, 0};  // L, L'
+  CUDA_TRY(c, cudaMemcpyAsync(counts, q->d_disc + SCALAR_WORDS, (size_t)npass * 8, cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(c, cudaStreamSynchronize(c->stream));
-  q->d2h_bytes += 8;
-  q->launches += 1;
+  const uint64_t live = counts[0];
+  q->canon_live = (uint32_t)counts[1];
+  q->d2h_bytes += npass * 8;
+  q->launches += npass;
   float ids_ms = 0;
   CUDA_TRY(c, cudaEventElapsedTime(&ids_ms, e0, e1));
   q->kernel_ms += ids_ms;
@@ -2754,6 +3066,11 @@ int discover_groups(sg_query* q, const std::vector<uint32_t>& list) {
   pool_release(c, q->d_acc);
   q->d_acc = nullptr;
   CUDA_TRY(c, pool_alloc(c, (void**)&q->d_acc, q->acc_words * 8));
+  if (q->dfold) {
+    pool_release(c, q->d_samples);
+    q->d_samples = nullptr;
+    CUDA_TRY(c, pool_alloc(c, (void**)&q->d_samples, std::max<size_t>(live, 1) * 16));
+  }
   point_plan(q);
   return SG_OK;
 }
@@ -3141,6 +3458,9 @@ static int build_result_topk(sg_query* q, sg_result** out, bool* fell_back) {
 // A row without the weight column reuses the previous row's weight (Q13, aggregate.go:68,100-102).  With
 // weight_carry the scan has already given such a row that weight's code, and a row left on code 0 had no earlier
 // row with the column in its block: weight 1, so the slot stays in place.  Without weight_carry it is refused.
+static const char* const NO_WEIGHT_MSG =
+    "query: rows without the weight column (the reference reuses the previous row's weight, aggregate.go:68,100-102): "
+    "not reproduced by this engine";
 static int fold_axes(sg_query* q, uint64_t* h, size_t have, sg_result* r, int64_t* matched_rows) {
   const Plan& P = q->plan;
   sg_ctx* c = q->ctx;
@@ -3164,8 +3484,7 @@ static int fold_axes(sg_query* q, uint64_t* h, size_t have, sg_result* r, int64_
         if (!cnt[s]) continue;
         const uint32_t code = (s / d.stride) % d.radix;
         if (code == 0 && !P.wcarry) {
-          c->set_err("query: rows without the weight column (the reference reuses the previous row's weight, "
-                     "aggregate.go:68,100-102): not reproduced by this engine");
+          c->set_err(NO_WEIGHT_MSG);
           return SG_ERR_UNSUPPORTED;
         }
         r->samples[s - code * d.stride] += cnt[s];
@@ -3222,6 +3541,39 @@ static int fold_axes(sg_query* q, uint64_t* h, size_t have, sg_result* r, int64_
   return SG_OK;
 }
 
+// A folded sparse plan's read-back: the scalars and, of every accumulator region, the rows of the L' canonical
+// groups (ids 0..L'-1), into a pinned buffer the result owns, laid out for L' rows.  The query's layout becomes
+// that one (the next run lays the accumulators out again after its discovery).
+static int read_canonical_rows(sg_query* q, sg_result* r) {
+  sg_ctx* c = q->ctx;
+  const uint32_t n = q->canon_live;
+  const size_t o_count = q->off_count;
+  const std::vector<size_t> o_sum = q->off_sum, o_hc = q->off_hcount, o_bk = q->off_buckets, o_max = q->off_vmax;
+  int rc = layout_accumulators(q, n);
+  if (rc != SG_OK) return rc;
+  q->plan.nslots = n;
+  r->pin = c->pin_get(q->acc_words * 8, &r->pin_bytes);
+  if (!r->pin) {
+    c->set_err("cudaHostAlloc (result buffer) failed");
+    return SG_ERR_CUDA;
+  }
+  uint64_t* h = (uint64_t*)r->pin;
+  auto back = [&](size_t to, size_t from, size_t words) {
+    return words ? cudaMemcpyAsync(h + to, q->d_acc + from, words * 8, cudaMemcpyDeviceToHost, c->stream) : cudaSuccess;
+  };
+  CUDA_TRY(c, back(0, 0, SCALAR_WORDS));
+  CUDA_TRY(c, back(q->off_count, o_count, n));
+  for (size_t a = 0; a < q->layouts.size(); a++) {
+    CUDA_TRY(c, back(q->off_sum[a], o_sum[a], n));
+    CUDA_TRY(c, back(q->off_hcount[a], o_hc[a], n));
+    CUDA_TRY(c, back(q->off_buckets[a], o_bk[a], (size_t)n * q->layouts[a].nvals_total));
+    CUDA_TRY(c, back(q->off_vmax[a], o_max[a], n));
+  }
+  CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+  q->d2h_bytes += (int64_t)q->acc_words * 8;
+  return SG_OK;
+}
+
 int build_result(sg_query* q, sg_result** out) {
   sg_ctx* c = q->ctx;
   const Plan& P = q->plan;
@@ -3250,7 +3602,13 @@ int build_result(sg_query* q, sg_result** out) {
   r->q = q;
   std::vector<uint64_t> hv;
   const uint64_t* h = nullptr;
-  if (q->h_pin_valid && q->h_pin) {  // read back behind the kernel into a pinned buffer: the result takes it over
+  if (q->sparse && q->dfold) {
+    // a folded sparse plan: the canonical groups hold ids 0..L'-1, and only their rows come back, laid out for L'
+    const int rc = read_canonical_rows(q, r.get());
+    if (rc != SG_OK) return rc;
+    have = q->acc_words;
+    h = (const uint64_t*)r->pin;
+  } else if (q->h_pin_valid && q->h_pin) {  // read back behind the kernel into a pinned buffer: the result takes it over
     r->pin = q->h_pin;
     r->pin_bytes = q->h_pin_bytes;
     q->h_pin = nullptr;
@@ -3280,8 +3638,12 @@ int build_result(sg_query* q, sg_result** out) {
       c->set_err("query: the hashed slot space filled up (more distinct group keys than its table holds)");
       return SG_ERR_UNSUPPORTED;
     }
-    if (!q->repl.empty() || q->d.weight_col_slot >= 0) {
+    if ((!q->repl.empty() || q->d.weight_col_slot >= 0) && !q->dfold) {
       c->set_err("query: StrReplace / weights over a hashed slot space are not in this build");
+      return SG_ERR_UNSUPPORTED;
+    }
+    if (q->dfold && h[3] != 0) {  // (fold_rows: rows left on weight code 0 without weight_carry)
+      c->set_err(NO_WEIGHT_MSG);
       return SG_ERR_UNSUPPORTED;
     }
     // slot -> key: the table itself, or for a sparse plan its id -> key array (L entries, nothing sized by the table)
@@ -3292,7 +3654,18 @@ int build_result(sg_query* q, sg_result** out) {
     q->d2h_bytes += (int64_t)P.nslots * 4;
   }
   int64_t w_rows = -1;  // weighted queries: matched ROWS (MatchedCount counts records, aggregate.go:117)
-  if (!q->repl.empty() || q->d.weight_col_slot >= 0) {
+  if (q->dfold) {
+    // folded on the device: a weighted result takes the rows per group the fold counted
+    if (q->d.weight_col_slot >= 0) {
+      r->samples.resize(P.nslots);
+      if (P.nslots)
+        CUDA_TRY(c, cudaMemcpyAsync(r->samples.data(), q->d_samples, (size_t)P.nslots * 8, cudaMemcpyDeviceToHost, c->stream));
+      CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+      q->d2h_bytes += (int64_t)P.nslots * 8;
+      w_rows = 0;
+      for (uint64_t n : r->samples) w_rows += (int64_t)n;
+    }
+  } else if (!q->repl.empty() || q->d.weight_col_slot >= 0) {
     if (q->merged && !q->repl.empty()) {
       c->set_err("query: StrReplace cannot follow a cross-GPU merge over differing dictionaries (seed them)");
       return SG_ERR_UNSUPPORTED;
@@ -3565,6 +3938,8 @@ void sg_query_free(sg_query* q) {
   if (q->h_pin) q->ctx->pin_put(q->h_pin, q->h_pin_bytes);
   if (q->ev0) cudaEventDestroy(q->ev0);
   if (q->ev1) cudaEventDestroy(q->ev1);
+  if (q->ev2) cudaEventDestroy(q->ev2);
+  if (q->ev3) cudaEventDestroy(q->ev3);
   delete q;
 }
 
@@ -3624,6 +3999,17 @@ int sg_query_set_sparse_groups(sg_query* q, int32_t on) {
   }
   if (on != q->sparse_req) q->planned = false;  // the next sg_query_run plans again
   q->sparse_req = on;
+  return SG_OK;
+}
+
+int sg_query_set_hashed_folds(sg_query* q, int32_t on) {
+  if (!q) return SG_ERR_INVALID;
+  if (on != 0 && on != 1) {
+    q->ctx->set_err("sg_query_set_hashed_folds: on must be 0 or 1");
+    return SG_ERR_INVALID;
+  }
+  if (on != q->hfold_req) q->planned = false;  // the next sg_query_run plans again
+  q->hfold_req = on;
   return SG_OK;
 }
 

@@ -44,6 +44,10 @@ class _Flags:
         # that occur only, as sybil's result map does (sg_query_set_sparse_groups).  False: such a query fails
         # with SG_ERR_UNSUPPORTED.
         self.SPARSE_GROUPS = False
+        # The engine's own flag: weighted and StrReplace group-bys whose keys go through the device hash table (or
+        # sparse group accumulators) are folded on the device (sg_query_set_hashed_folds).  False: such a query fails
+        # with SG_ERR_UNSUPPORTED.
+        self.HASHED_FOLDS = False
 
 
 FLAGS = _Flags()
@@ -521,6 +525,8 @@ class PreparedQuery:
         try:
             if FLAGS.SPARSE_GROUPS:
                 ctx.check(lib.sg_query_set_sparse_groups(self.q, 1))
+            if FLAGS.HASHED_FOLDS:
+                ctx.check(lib.sg_query_set_hashed_folds(self.q, 1))
             for name, strs in rewritten.items():
                 blob = b"".join(strs)
                 offs = np.zeros(len(strs) + 1, np.uint32)
