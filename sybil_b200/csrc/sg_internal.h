@@ -85,6 +85,28 @@ struct DevBlock {
 // ---- query plan (device copy read by the kernels) ---------------------------------
 constexpr int MAX_SUBHISTS = 64;
 
+// The scalar words that open the accumulator array (Plan::scalars).  All of them lie in the region a cross-GPU merge
+// sums.  A nonzero time overflow, rows on weight code 0, table full or sparse key missing fails the query.
+enum : uint32_t {
+  SC_MATCHED = 0,         // rows that passed every filter (scan)
+  SC_BROKEN = 1,          // blocks the scan found broken (scan)
+  SC_TIME_OVERFLOW = 2,   // rows outside the planned time axis (scan)
+  SC_NO_WEIGHT = 3,       // weighted folds: rows left on weight code 0 without weight_carry
+  SC_TABLE_FULL = 4,      // hashed slot space: inserts that found the table full (scan, fold_insert)
+  SC_SPARSE_MISSING = 5,  // sparse plans: rows whose key the aggregation launch did not find (scan)
+  SC_FOLD_ENTRIES = 6,    // device folds: the table's occupied entries (fold_rows)
+  SC_FOLD_CANON = 7,      // ... the canonical ones among them (fold_rows)
+  // the cross-GPU merge header (sg_query_allreduce, cleared again after the merge): broken staged blocks, skipped
+  // blocks, rows scanned, blocks scanned, then four words that check the ranks' axes agree
+  SC_MERGE = 8,
+  SC_MERGE_AXES = 12,
+  SCALAR_WORDS = 16,
+  // a sparse plan's discovery launch writes its scalars to an array of its own, followed by two counters (assign_ids):
+  DISC_LIVE = SCALAR_WORDS,  // the table's occupied entries, which get the ids 0..live-1
+  DISC_CANON,                // device folds: the canonical entries among them (ids 0..canon-1)
+  DISC_WORDS
+};
+
 struct KFilter {
   int32_t col;
   int32_t is_str;
@@ -181,7 +203,7 @@ struct Plan {
   uint32_t hist_rows;
   uint32_t hist_row_words;
   uint64_t* count;      // [nslots]
-  uint64_t* scalars;    // [0] matched rows, [1] broken blocks, [2] time overflow rows, [3] blocks done
+  uint64_t* scalars;    // [SCALAR_WORDS] (SC_*)
   uint32_t* block_status;  // per table block: 1 = broken in this query
   KFilter filters[SG_MAX_FILTERS];
   KGroup groups[SG_MAX_GROUPS];
@@ -213,14 +235,14 @@ struct LaunchParams {
   // mixed-radix code (< 2^31) is looked up / inserted in this open-addressing table (key = code + 1, 0 = empty) and the
   // slot word's group bits are replaced by the table index, which is what the accumulators are indexed by
   // (plan.nslots == hmask + 1; a sparse plan's accumulators are indexed by hids below, plan.nslots == its live groups,
-  // and the table has hmask + 1 entries all the same).  nullptr: the slot space is dense.  scalars[4] counts rows that
+  // and the table has hmask + 1 entries all the same).  nullptr: the slot space is dense.  SC_TABLE_FULL counts rows that
   // found the table full.
   uint32_t* hkeys;
   uint32_t hmask;
   // Sparse group accumulators (sg_query_set_sparse_groups): the same table is filled by a discovery launch
   // (hdisc = 1: codes are inserted, nothing is counted or aggregated), then each occupied entry gets a dense id
   // (assign_ids), then the aggregation launch (hids != nullptr) looks every code up without inserting and writes
-  // hids[index] into the slot word's group bits.  The accumulators are indexed by that id.  scalars[5] counts rows
+  // hids[index] into the slot word's group bits.  The accumulators are indexed by that id.  SC_SPARSE_MISSING counts rows
   // whose code the aggregation launch did not find (an internal inconsistency that fails the query).
   const uint32_t* hids;
   uint32_t hdisc;

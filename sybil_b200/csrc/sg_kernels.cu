@@ -1731,7 +1731,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
                 sred_add(smem_u32(cx.acc + p * gstride + lane_off), c.bin_offsets[b + 1] - c.bin_offsets[b]);
             } else {
               const uint32_t rc = rel_of(time_code(c.bin_values[b], tbk, tfirst, tradix));
-              p = rc ? rc * tstride + time_ok : 0u;  // 0: counted into scalars[2] below
+              p = rc ? rc * tstride + time_ok : 0u;  // 0: counted into SC_TIME_OVERFLOW below
             }
           }
           pay[b] = p;
@@ -1795,7 +1795,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
             reinterpret_cast<uint4*>(slot + idx0)[j] = make_uint4(w[4 * j], w[4 * j + 1], w[4 * j + 2], w[4 * j + 3]);
         }
       }
-      if (ovf) gred_add(g_scalars + 2, ovf);
+      if (ovf) gred_add(g_scalars + SC_TIME_OVERFLOW, ovf);
       __syncthreads();
       pass_mark(pass_no++);
     }
@@ -2027,7 +2027,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
     // ---- time bucket (aggregate.go:146-183) ------------------------------------------
     // The slot word takes the code relative to the block's window (1..twin; see Plan).  A row outside
     // the planned axis — or outside the window, which the exact extents rule out — is counted in
-    // scalars[2] and fails the query on the host.
+    // SC_TIME_OVERFLOW and fails the query on the host.
     const bool time_pass = time_col >= 0 && !(ptmp[4 * (nfilters + ngroups)] & 2u);  // (else read in the code pass)
     if (time_pass) {
       const DevCol c = colcache[nfilters + ngroups];
@@ -2075,7 +2075,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
               if (cur)
                 slot_add(slot, slot_s, row, cur * ts + (uint32_t)tok);
               else
-                gred_add(g_scalars + 2, 1ull);
+                gred_add(g_scalars + SC_TIME_OVERFLOW, 1ull);
             });
       } else if (c.enc == SG_ENC_VALUES && !(c.flags & COL_IS_STR)) {
         const bool stats = (c.flags & COL_STATS) != 0;
@@ -2098,7 +2098,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
                 if (rc)
                   inc[k] = rc * ts + time_ok;
                 else
-                  gred_add(g_scalars + 2, 1ull);
+                  gred_add(g_scalars + SC_TIME_OVERFLOW, 1ull);
               }
             }
             add_slots(slot, idx0, inc);
@@ -2114,7 +2114,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
                 if (rc)
                   inc[k] = rc * ts + time_ok;
                 else
-                  gred_add(g_scalars + 2, 1ull);
+                  gred_add(g_scalars + SC_TIME_OVERFLOW, 1ull);
               }
             }
             add_slots(slot, idx0, inc);
@@ -2153,8 +2153,8 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
               idx = __ldg(hids + idx);
               break;
             }
-            if (k == 0u || ++probes > hmask) {  // not discovered: the host fails the query (scalars[5])
-              gred_add(g_scalars + 5, 1ull);
+            if (k == 0u || ++probes > hmask) {  // not discovered: the host fails the query (SC_SPARSE_MISSING)
+              gred_add(g_scalars + SC_SPARSE_MISSING, 1ull);
               idx = 0u;
               break;
             }
@@ -2165,8 +2165,8 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
             const uint32_t old = atomicCAS(hk + idx, 0u, key);
             if (old == 0u || old == key) break;
             idx = (idx + 1u) & hmask;
-            if (++probes > hmask) {  // table full: the host fails the query (scalars[4])
-              gred_add(g_scalars + 4, 1ull);
+            if (++probes > hmask) {  // table full: the host fails the query (SC_TABLE_FULL)
+              gred_add(g_scalars + SC_TABLE_FULL, 1ull);
               idx = 0u;
               break;
             }
@@ -2626,7 +2626,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
     if (broken) {
       if (cx.tid == 0) {
         PP->block_status[bid] = 1;
-        gred_add(g_scalars + 1, 1ull);
+        gred_add(g_scalars + SC_BROKEN, 1ull);
       }
     } else {
       if (owner) matched += my_matched;
@@ -2668,7 +2668,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) scan_kernel(const Launch
   // MatchedCount
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) matched += __shfl_xor_sync(FULL, matched, d);
-  if (cx.lane == 0 && matched) gred_add(g_scalars + 0, matched);
+  if (cx.lane == 0 && matched) gred_add(g_scalars + SC_MATCHED, matched);
 }
 
 // ---------------------------------------------------------------------------

@@ -1307,10 +1307,11 @@ struct GroupDim {  // one axis of the dense slot space
   uint32_t radix = 1, stride = 1;
 };
 
-// The canonical key of a table entry (device folds, sg_query_set_hashed_folds): the entry's code with the weight
-// digit set to 0 and each rewritten axis' digit replaced by its class representative's (0 when the string rewrites
-// to "": the missing group, DESIGN.md §7); every other digit, time included, unchanged.  What fold_axes does per
-// dense slot, restated per key.
+// The canonical key of a group code (canon_code), the one definition of the weight and StrReplace folds: the code
+// with the weight digit set to 0 and each rewritten axis' digit replaced by its class representative's (0 when the
+// string rewrites to "": the missing group, DESIGN.md §7); every other digit, time included, unchanged.  Dense plans
+// fold their slots on the host (dense_fold), hashed and sparse plans their table entries on the device (fold_rows);
+// build_fold_key fills it, with the tables in host vectors the caller points it at.
 struct FoldKey {
   uint32_t naxes = 0;  // rewritten (StrReplace) axes
   uint32_t stride[SG_MAX_GROUPS] = {}, radix[SG_MAX_GROUPS] = {};
@@ -1319,6 +1320,14 @@ struct FoldKey {
   uint32_t wcarry = 0;
   const int64_t* wmul = nullptr;     // per weight code its multiplier (code 0: weight 1 under wcarry)
   const uint32_t* luts = nullptr;    // per rewritten axis, radix entries: digit -> canonical digit
+};
+
+// One region of the accumulator array after the scalars (layout_accumulators): per row `per_row` words at `off`,
+// merged and folded by addition, or by max (the MAX region)
+struct AccRegion {
+  size_t off;
+  uint32_t per_row;
+  bool is_max;
 };
 
 struct ResultGroup {
@@ -1403,6 +1412,7 @@ struct sg_query {
   size_t prefix_words = 0;  // scalars | count | sums
   size_t off_count = 0;
   std::vector<size_t> off_hcount, off_sum, off_vmax, off_buckets;
+  std::vector<AccRegion> regions;  // the regions above in layout order (bucket counters of no width left out)
   uint32_t* d_block_status = nullptr;
   uint32_t* d_block_list = nullptr;
   uint32_t* d_item_mask = nullptr;
@@ -1447,7 +1457,7 @@ struct sg_query {
   int32_t sparse_req = 0;        // the setter's value, applied by the next plan
   bool sparse = false;           // this plan takes the path
   uint32_t* d_hids = nullptr;    // [hcap] table entry -> dense id, then [hcap] dense id -> key (code + 1)
-  uint64_t* d_disc = nullptr;    // the discovery launch's scalars (SCALAR_WORDS), then the live and canonical counts
+  uint64_t* d_disc = nullptr;    // [DISC_WORDS] the discovery launch's scalars, then the live and canonical counts
   double disc_ms = 0;            // the last discovery launch (SG_PLAN_TRACE)
   // device folds (sg_query_set_hashed_folds): a hashed or sparse plan with weights or StrReplace combines the
   // accumulators of every table entry onto its canonical entry on the device (fold_insert, fold_rows)
@@ -1719,9 +1729,9 @@ int ensure_value_dict(sg_table* t, int col) {
   return SG_OK;
 }
 
-// scalars: [0] matched rows, [1] broken blocks, [2] time overflow rows (kernel); [8..15] the cross-GPU
-// merge header (block counters + axes signature) written by sg_query_allreduce
-constexpr size_t SCALAR_WORDS = 16;
+// The accumulator array: SCALAR_WORDS scalars (SC_* in sg_internal.h), then per slot regions in this order: count,
+// the exact sums, the hist Counts, the bucket counters (all added when merged or folded: the SUM region), then the
+// max above info_max (the MAX region).  q->regions lists them; the off_* members name them one by one.
 constexpr uint64_t ACC_LIMIT_BYTES = (uint64_t)24 << 30;
 // bytes of the SUM region (scalars | count | sums | hist Counts | bucket counters) for nslots slots: what the
 // 24 GiB limit of layout_accumulators is taken on
@@ -1732,27 +1742,26 @@ static uint64_t sum_region_bytes(const sg_query* q, uint64_t nslots) {
 }
 int layout_accumulators(sg_query* q, uint32_t nslots) {
   const int naggs = (int)q->layouts.size();
-  size_t words = SCALAR_WORDS;  // scalars
-  q->off_count = words;
-  words += nslots;
+  size_t words = SCALAR_WORDS;
   q->off_hcount.clear();
   q->off_sum.clear();
   q->off_vmax.clear();
   q->off_buckets.clear();
+  q->regions.clear();
+  auto region = [&](uint32_t per_row, bool is_max) {
+    const size_t off = words;
+    if (per_row) q->regions.push_back({off, per_row, is_max});
+    words += (size_t)nslots * per_row;
+    return off;
+  };
+  q->off_count = region(1, false);
   // all sums, then all hist Counts: when every hist Count equals Count (hc_is_count) and no buckets exist,
   // scalars | count | sums is all a result needs and it is one contiguous prefix of the array
-  for (int i = 0; i < naggs; i++) {
-    q->off_sum.push_back(words);
-    words += nslots;
-  }
+  for (int i = 0; i < naggs; i++) q->off_sum.push_back(region(1, false));
   q->prefix_words = words;
+  for (int i = 0; i < naggs; i++) q->off_hcount.push_back(region(1, false));
   for (int i = 0; i < naggs; i++) {
-    q->off_hcount.push_back(words);
-    words += nslots;
-  }
-  for (int i = 0; i < naggs; i++) {
-    q->off_buckets.push_back(words);
-    words += (size_t)nslots * q->layouts[(size_t)i].nvals_total;
+    q->off_buckets.push_back(region(q->layouts[(size_t)i].nvals_total, false));
     if (words * 8 > ACC_LIMIT_BYTES) {
       q->ctx->set_err("query: accumulators exceed 24 GiB (groups x histogram buckets); needs sparse group "
                       "accumulators (sg_query_set_sparse_groups)");
@@ -1760,10 +1769,7 @@ int layout_accumulators(sg_query* q, uint32_t nslots) {
     }
   }
   q->sum_words = words;
-  for (int i = 0; i < naggs; i++) {
-    q->off_vmax.push_back(words);
-    words += nslots;
-  }
+  for (int i = 0; i < naggs; i++) q->off_vmax.push_back(region(1, true));
   q->acc_words = words;
   return SG_OK;
 }
@@ -1787,7 +1793,7 @@ int make_plan(sg_query* q, const std::vector<uint32_t>& list) {
   // Weighted queries (OPTS.WEIGHT_COL, aggregate.go:68,100-102,202-203; hist_basic.go:111-151): Count += weight,
   // hist Count += weight, Values[bucket] += weight, mean weighted.  All of these are linear in the weight, so the
   // scan groups by the weight VALUE as one more (hidden, last) axis — the ordinary int group-by — and the host
-  // folds that axis away with a multiplication per slot (fold_axes).  Rows WITHOUT the weight column reuse the
+  // folds that axis away with a multiplication per slot (dense_fold).  Rows WITHOUT the weight column reuse the
   // previous row's weight in the reference (Q13): with weight_carry the scan fills their digit of the weight axis
   // forward from the nearest earlier row of the block (a row with no such row keeps code 0: weight 1); without it
   // such a query is refused when the result is built.
@@ -1961,7 +1967,7 @@ int make_plan(sg_query* q, const std::vector<uint32_t>& list) {
     hashed = true;
   }
   q->hashed = hashed;
-  // ---- device folds (sg_query_set_hashed_folds): a hashed slot space has no slot arithmetic for fold_axes, so its
+  // ---- device folds (sg_query_set_hashed_folds): a hashed slot space has no slot per code for dense_fold, so its
   // weight axis and rewritten strings are folded over the table's entries on the device (fold_insert, fold_rows)
   q->dfold = hashed && q->hfold_req == 1 && (weighted || !q->repl.empty());
   if (stride > (uint64_t)MAX_SLOTS && !q->hashed) {
@@ -2317,7 +2323,7 @@ int alloc_device(sg_query* q) {
   if (q->hashed) CUDA_TRY(c, pool_alloc(c, (void**)&q->d_hkeys, (size_t)q->hcap * 4));
   if (q->sparse) {
     CUDA_TRY(c, pool_alloc(c, (void**)&q->d_hids, (size_t)q->hcap * 8));
-    if (!q->d_disc) CUDA_TRY(c, pool_alloc(c, (void**)&q->d_disc, (SCALAR_WORDS + 2) * 8));
+    if (!q->d_disc) CUDA_TRY(c, pool_alloc(c, (void**)&q->d_disc, DISC_WORDS * 8));
   }
   if (!q->ev0) {
     CUDA_TRY(c, cudaEventCreate(&q->ev0));
@@ -2339,40 +2345,50 @@ int alloc_device(sg_query* q) {
   return SG_OK;
 }
 
-// The device fold's tables (FoldKey): the weight axis' multipliers and each rewritten axis' digit -> canonical digit
-// map, from the same dictionaries and StrReplace classes fold_axes reads
-int upload_fold(sg_query* q) {
+// The plan's canonical key (FoldKey) without its table pointers: the weight axis' multipliers (wmul: code 0 -> 1, then
+// the weight dictionary, the union one after a cross-GPU merge) and each rewritten axis' digit -> canonical digit map
+// (luts), from the dictionaries and StrReplace classes as they are now.  Refused if those no longer match the plan.
+static int build_fold_key(sg_query* q, FoldKey* F, std::vector<int64_t>* wmul, std::vector<uint32_t>* luts) {
   sg_ctx* c = q->ctx;
-  FoldKey& F = q->fkey;
-  F = FoldKey();
-  F.wcarry = q->plan.wcarry;
-  std::vector<int64_t> wmul;
-  std::vector<uint32_t> luts;
-  for (const GroupDim& d : q->dims) {
+  *F = FoldKey();
+  F->wcarry = q->plan.wcarry;
+  for (size_t di = 0; di < q->dims.size(); di++) {
+    const GroupDim& d = q->dims[di];
     if (d.is_weight) {
-      const std::vector<int64_t>& vals = q->table->idict[(size_t)d.col].vals;
+      const std::vector<int64_t>& vals = q->merged ? q->m_ints[di] : q->table->idict[(size_t)d.col].vals;
       if (vals.size() + 1 != (size_t)d.radix) {
         c->set_err("query: the weight column's value dictionary changed under the query");
         return SG_ERR_STATE;
       }
-      F.wstride = d.stride;
-      F.wradix = d.radix;
-      wmul.push_back(1);
-      wmul.insert(wmul.end(), vals.begin(), vals.end());
+      F->wstride = d.stride;
+      F->wradix = d.radix;
+      wmul->push_back(1);
+      wmul->insert(wmul->end(), vals.begin(), vals.end());
     } else if (d.is_str && q->repl.count(d.col)) {
       const auto& R = q->repl.at(d.col);
       if (R.canon.size() + 1 != (size_t)d.radix || R.strs.size() != R.canon.size()) {
         c->set_err("query: the dictionary of a StrReplace column grew after sg_query_set_str_replace");
         return SG_ERR_STATE;
       }
-      F.stride[F.naxes] = d.stride;
-      F.radix[F.naxes] = d.radix;
-      F.lut[F.naxes] = (uint32_t)luts.size();
-      F.naxes++;
-      luts.push_back(0);
-      for (size_t i = 0; i < R.canon.size(); i++) luts.push_back(R.strs[i].empty() ? 0u : R.canon[i] + 1u);
+      F->stride[F->naxes] = d.stride;
+      F->radix[F->naxes] = d.radix;
+      F->lut[F->naxes] = (uint32_t)luts->size();
+      F->naxes++;
+      luts->push_back(0);
+      for (size_t i = 0; i < R.canon.size(); i++) luts->push_back(R.strs[i].empty() ? 0u : R.canon[i] + 1u);
     }
   }
+  return SG_OK;
+}
+
+// the device fold's key, its tables copied to d_fold
+int upload_fold(sg_query* q) {
+  sg_ctx* c = q->ctx;
+  FoldKey& F = q->fkey;
+  std::vector<int64_t> wmul;
+  std::vector<uint32_t> luts;
+  const int rc = build_fold_key(q, &F, &wmul, &luts);
+  if (rc != SG_OK) return rc;
   const size_t wbytes = wmul.size() * 8, bytes = wbytes + luts.size() * 4;
   pool_release(c, q->d_fold);
   q->d_fold = nullptr;
@@ -2743,7 +2759,7 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list, bool discover = fal
   CUDA_TRY(c, cudaMemcpyAsync(back, discover ? q->d_disc : q->d_acc, acc_back, cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(c, cudaStreamSynchronize(c->stream));
   if (back == q->h_pin) {
-    q->h_acc.assign((const uint64_t*)back, (const uint64_t*)back + 8);  // the scalars (sg_query_run reads them)
+    q->h_acc.assign((const uint64_t*)back, (const uint64_t*)back + SC_MERGE);  // the scalars (sg_query_run reads them)
     q->h_acc_valid = false;
     q->h_pin_valid = true;
   } else {
@@ -2763,10 +2779,10 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list, bool discover = fal
     q->kernel_ms += ims + fms;
     if (discover || !q->sparse) q->insert_ms = ims;
     q->fold_ms = fms;
-    // scalars [6] / [7]: the table's occupied entries / the canonical ones among them (fold_rows)
     if (!discover && getenv("SG_PLAN_TRACE"))
-      fprintf(stderr, "sg_fold: entries=%llu canon=%llu insert_ms=%.4f fold_ms=%.4f\n", (unsigned long long)q->h_acc[6],
-              (unsigned long long)q->h_acc[7], q->insert_ms, q->fold_ms);
+      fprintf(stderr, "sg_fold: entries=%llu canon=%llu insert_ms=%.4f fold_ms=%.4f\n",
+              (unsigned long long)q->h_acc[SC_FOLD_ENTRIES], (unsigned long long)q->h_acc[SC_FOLD_CANON], q->insert_ms,
+              q->fold_ms);
   }
   if (d_dbg) {
     std::vector<unsigned long long> hd((size_t)q->grid * 16);
@@ -2791,7 +2807,7 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list, bool discover = fal
   return SG_OK;
 }
 
-__device__ __forceinline__ uint32_t canon_code(const FoldKey& F, uint32_t code) {
+__host__ __device__ __forceinline__ uint32_t canon_code(const FoldKey& F, uint32_t code) {
   uint32_t out = code;
 #pragma unroll
   for (uint32_t a = 0; a < SG_MAX_GROUPS; a++) {  // (unrolled: the parameter arrays stay out of local memory)
@@ -2832,7 +2848,7 @@ __global__ void assign_ids(const uint32_t* __restrict__ keys, uint32_t cap, uint
 // Canonical insert: every occupied entry whose key is not canonical inserts its canonical key into the same table,
 // with the scan's probing (a hashed plan: after the scan; a sparse plan: after discovery, so that the canonical
 // entries get ids and accumulator rows).  An entry read while another thread inserts it is canonical: nothing to
-// do.  scalars[4] counts inserts that found the table full, as the scan does.
+// do.  SC_TABLE_FULL counts inserts that found the table full, as the scan does.
 __global__ void fold_insert(uint32_t* hk, uint32_t hmask, FoldKey F, unsigned long long* scalars) {
   const uint32_t stride = gridDim.x * blockDim.x;
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i <= hmask; i += stride) {
@@ -2846,7 +2862,7 @@ __global__ void fold_insert(uint32_t* hk, uint32_t hmask, FoldKey F, unsigned lo
       if (old == 0u || old == key) break;
       idx = (idx + 1u) & hmask;
       if (++probes > hmask) {
-        atomicAdd(scalars + 4, 1ull);
+        atomicAdd(scalars + SC_TABLE_FULL, 1ull);
         break;
       }
     }
@@ -2870,11 +2886,10 @@ struct FoldAcc {
 };
 
 // Fold: every non-canonical entry e with canonical entry c and weight multiplier w adds acc[e] * w into acc[c]
-// (uint64, wrapping: fold_axes' arithmetic) and takes the max into the MAX region unmultiplied, then clears e; its
+// (uint64, wrapping: dense_fold's arithmetic) and takes the max into the MAX region unmultiplied, then clears e; its
 // rows go to samples[c], where a canonical entry's own rows also land.  Integer sums in any order: the result is
 // the dense path's bit for bit.  Each warp reads 32 entries, then folds its sources one after the other with the
-// lanes striding over the source's words.  scalars: [3] rows on weight code 0 without carry (refused), [6] occupied
-// entries, [7] canonical ones.
+// lanes striding over the source's words.  Scalars: SC_NO_WEIGHT, SC_FOLD_ENTRIES, SC_FOLD_CANON.
 __global__ void fold_rows(FoldAcc A, FoldKey F) {
   const uint32_t lane = threadIdx.x & 31u;
   const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
@@ -2892,7 +2907,7 @@ __global__ void fold_rows(FoldAcc A, FoldKey F) {
       uint32_t to = row;
       if (F.wradix) {
         const uint32_t wd = (code / F.wstride) % F.wradix;
-        if (wd == 0u && !F.wcarry && own) atomicAdd(A.scalars + 3, own);
+        if (wd == 0u && !F.wcarry && own) atomicAdd(A.scalars + SC_NO_WEIGHT, own);
         mul = (unsigned long long)F.wmul[wd];
       }
       canon = cc == code;
@@ -2917,8 +2932,8 @@ __global__ void fold_rows(FoldAcc A, FoldKey F) {
     }
     const unsigned occ = __ballot_sync(0xffffffffu, k != 0u), can = __ballot_sync(0xffffffffu, canon);
     if (lane == 0 && occ) {
-      atomicAdd(A.scalars + 6, (unsigned long long)__popc(occ));
-      if (can) atomicAdd(A.scalars + 7, (unsigned long long)__popc(can));
+      atomicAdd(A.scalars + SC_FOLD_ENTRIES, (unsigned long long)__popc(occ));
+      if (can) atomicAdd(A.scalars + SC_FOLD_CANON, (unsigned long long)__popc(can));
     }
     for (unsigned m = __ballot_sync(0xffffffffu, src != NONE); m; m &= m - 1u) {
       const int l = __ffs((int)m) - 1;
@@ -2980,15 +2995,16 @@ int device_fold(sg_query* q, bool discover) {
     A.samples = (unsigned long long*)q->d_samples;
     A.own = (const unsigned long long*)(q->d_samples + n);
     A.scalars = scalars;
-    A.add_off[A.nadd++] = q->off_count;
-    for (int a = 0; a < P.naggs; a++) {
-      A.add_off[A.nadd++] = q->off_sum[(size_t)a];
-      A.add_off[A.nadd++] = q->off_hcount[(size_t)a];
-      A.max_off[A.nmax++] = q->off_vmax[(size_t)a];
-      const uint32_t nv = q->layouts[(size_t)a].nvals_total;
-      if (nv) {
-        A.bk_off[A.nbk] = q->off_buckets[(size_t)a];
-        A.bk_nv[A.nbk++] = nv;
+    // (the one-word added regions, count, sums and hist Counts, come first and fit add_off; a bucket region
+    // that is one word wide may follow them there while room is left)
+    for (const AccRegion& R : q->regions) {
+      if (R.is_max) {
+        A.max_off[A.nmax++] = R.off;
+      } else if (R.per_row == 1 && A.nadd < 1 + 2 * SG_MAX_AGGS) {
+        A.add_off[A.nadd++] = R.off;
+      } else {
+        A.bk_off[A.nbk] = R.off;
+        A.bk_nv[A.nbk++] = R.per_row;
       }
     }
     CUDA_TRY(c, cudaMemsetAsync(q->d_samples, 0, n * 8, c->stream));
@@ -3009,24 +3025,24 @@ int discover_groups(sg_query* q, const std::vector<uint32_t>& list) {
   sg_ctx* c = q->ctx;
   Plan& P = q->plan;
   CUDA_TRY(c, cudaMemsetAsync(q->d_hkeys, 0, (size_t)q->hcap * 4, c->stream));
-  CUDA_TRY(c, cudaMemsetAsync(q->d_disc, 0, (SCALAR_WORDS + 2) * 8, c->stream));
+  CUDA_TRY(c, cudaMemsetAsync(q->d_disc, 0, DISC_WORDS * 8, c->stream));
   uint64_t* const acc_scalars = P.scalars;
   P.scalars = q->d_disc;
   int rc = run_list(q, list, true);
   P.scalars = acc_scalars;
   if (rc != SG_OK) return rc;
   const uint64_t* scal = q->h_acc.data();
-  if (scal[2] != 0) {
+  if (scal[SC_TIME_OVERFLOW] != 0) {
     c->set_err("query: rows fall outside the planned time axis (time_min/time_max too narrow)");
     return SG_ERR_INVALID;
   }
-  if (scal[4] != 0) {
+  if (scal[SC_TABLE_FULL] != 0) {
     c->set_err("query: the hashed slot space filled up (more distinct group keys than its table holds)");
     return SG_ERR_UNSUPPORTED;
   }
   uint32_t* const d_ids = q->d_hids;
   uint32_t* const d_id2key = q->d_hids + q->hcap;
-  unsigned int* const d_live = reinterpret_cast<unsigned int*>(q->d_disc + SCALAR_WORDS);
+  unsigned int* const d_live = reinterpret_cast<unsigned int*>(q->d_disc + DISC_LIVE);
   cudaEvent_t e0 = q->ev0, e1 = q->ev1;
   CUDA_TRY(c, cudaEventRecord(e0, c->stream));
   const unsigned grid = (unsigned)std::min<uint64_t>(((uint64_t)q->hcap + 255) / 256, (uint64_t)std::max(c->sm_count, 1) * 8);
@@ -3036,11 +3052,11 @@ int discover_groups(sg_query* q, const std::vector<uint32_t>& list) {
     assign_ids<<<grid, 256, 0, c->stream>>>(q->d_hkeys, q->hcap, d_ids, d_id2key, d_live, q->fkey, q->dfold ? pass + 1 : 0);
     CUDA_TRY(c, cudaGetLastError());
     if (q->dfold && pass == 0)
-      CUDA_TRY(c, cudaMemcpyAsync(q->d_disc + SCALAR_WORDS + 1, q->d_disc + SCALAR_WORDS, 8, cudaMemcpyDeviceToDevice, c->stream));
+      CUDA_TRY(c, cudaMemcpyAsync(q->d_disc + DISC_CANON, q->d_disc + DISC_LIVE, 8, cudaMemcpyDeviceToDevice, c->stream));
   }
   CUDA_TRY(c, cudaEventRecord(e1, c->stream));
   uint64_t counts[2] = {0, 0};  // L, L'
-  CUDA_TRY(c, cudaMemcpyAsync(counts, q->d_disc + SCALAR_WORDS, (size_t)npass * 8, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(c, cudaMemcpyAsync(counts, q->d_disc + DISC_LIVE, (size_t)npass * 8, cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(c, cudaStreamSynchronize(c->stream));
   const uint64_t live = counts[0];
   q->canon_live = (uint32_t)counts[1];
@@ -3324,7 +3340,7 @@ static int build_result_topk(sg_query* q, sg_result** out, bool* fell_back) {
   CUDA_TRY(c, cudaMemcpyAsync(dp + off_offs, hp + off_offs, 512, cudaMemcpyHostToDevice, c->stream));
   topk_totals<<<grid, 256, 0, c->stream>>>(A, naggs, d_off_hc, d_off_sum, d_hcic, d_tot);
   CUDA_TRY(c, cudaMemcpyAsync(hp + off_tot, d_tot, sizeof(TopkTotals), cudaMemcpyDeviceToHost, c->stream));
-  CUDA_TRY(c, cudaMemcpyAsync(hp + off_scal, q->d_acc, 128, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(c, cudaMemcpyAsync(hp + off_scal, q->d_acc, SCALAR_WORDS * 8, cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(c, cudaStreamSynchronize(c->stream));
   q->launches += 1;
   TopkTotals T = *(const TopkTotals*)(hp + off_tot);
@@ -3414,7 +3430,7 @@ static int build_result_topk(sg_query* q, sg_result** out, bool* fell_back) {
   r->hist_mode = false;
   r->ngroups_cols = (int)q->groups.size();
   r->naggs = naggs;
-  r->broken = q->broken_staged + (int64_t)scal[1];
+  r->broken = q->broken_staged + (int64_t)scal[SC_BROKEN];
   r->skipped = q->skipped;
   init_group(r->total, naggs);
   r->total.skey = "TOTAL";
@@ -3444,15 +3460,15 @@ static int build_result_topk(sg_query* q, sg_result** out, bool* fell_back) {
   return SG_OK;
 }
 
-// Host-side folds of the dense accumulators before the result is built.
+// The folds of the accumulators before the result is built (canon_code: dense_fold here, fold_rows on the device).
 //
 // StrReplace: strings of a group column that rewrite to the same text are one group in the reference (the block's
 // string table is rewritten before any row is read, column_store_io.go:529-547).  The scan grouped by the original
-// global ids; every dense slot whose code on a rewritten axis is not its class representative is added onto the
-// representative's slot (counts, hist counts, sums, bucket counters: +; max: max) and cleared.  A string that
+// global ids; every group whose code on a rewritten axis is not its class representative is added onto the
+// representative's group (counts, hist counts, sums, bucket counters: +; max: max) and cleared.  A string that
 // rewrites to "" goes onto code 0 instead: it renders like a missing value, and is the missing group (DESIGN.md §7).
 //
-// Weights (OPTS.WEIGHT_COL): the scan grouped by the weight value as a hidden last axis (make_plan); the slots of
+// Weights (OPTS.WEIGHT_COL): the scan grouped by the weight value as a hidden last axis (make_plan); the groups of
 // weight w are multiplied by w and added onto code 0 of that axis — Count / hist Count / Values[] += weight
 // (aggregate.go:203, hist_basic.go:111-116,146), exact sum += value * weight; Result.Samples keeps the rows.
 // A row without the weight column reuses the previous row's weight (Q13, aggregate.go:68,100-102).  With
@@ -3461,84 +3477,43 @@ static int build_result_topk(sg_query* q, sg_result** out, bool* fell_back) {
 static const char* const NO_WEIGHT_MSG =
     "query: rows without the weight column (the reference reuses the previous row's weight, aggregate.go:68,100-102): "
     "not reproduced by this engine";
-static int fold_axes(sg_query* q, uint64_t* h, size_t have, sg_result* r, int64_t* matched_rows) {
-  const Plan& P = q->plan;
-  sg_ctx* c = q->ctx;
-  for (size_t di = 0; di < q->dims.size(); di++) {
-    const GroupDim& d = q->dims[di];
-    if (d.is_time) continue;
-    const std::vector<uint32_t>* canon = nullptr;
-    const std::vector<std::string>* rtext = nullptr;  // StrReplace: the rewritten text of every global id
-    std::vector<uint64_t> wmul;  // weight axis: multiplier per code - 1
-    if (d.is_weight) {
-      const std::vector<int64_t>& vals = q->merged ? q->m_ints[di] : q->table->idict[(size_t)d.col].vals;
-      if (vals.size() + 1 != (size_t)d.radix) {
-        c->set_err("query: the weight column's value dictionary changed under the query");
-        return SG_ERR_STATE;
-      }
-      wmul.assign(vals.begin(), vals.end());
-      const uint64_t* cnt = h + q->off_count;
-      r->samples.assign(P.nslots, 0);
-      int64_t rows = 0;
-      for (uint32_t s = 0; s < P.nslots; s++) {
-        if (!cnt[s]) continue;
-        const uint32_t code = (s / d.stride) % d.radix;
-        if (code == 0 && !P.wcarry) {
-          c->set_err(NO_WEIGHT_MSG);
-          return SG_ERR_UNSUPPORTED;
-        }
-        r->samples[s - code * d.stride] += cnt[s];
-        rows += (int64_t)cnt[s];
-      }
-      if (matched_rows) *matched_rows = rows;
-    } else if (d.is_str) {
-      auto it = q->repl.find(d.col);
-      if (it == q->repl.end()) continue;
-      canon = &it->second.canon;
-      rtext = &it->second.strs;
-      if (canon->size() + 1 != (size_t)d.radix || rtext->size() != canon->size()) {
-        c->set_err("query: the dictionary of a StrReplace column grew after sg_query_set_str_replace");
-        return SG_ERR_STATE;
-      }
-    } else {
-      continue;
+
+// The dense plans' fold (the device's is fold_rows, over table entries): every slot s moves onto its canonical slot
+// c = canon_code(F, s) with its weight multiplier w: acc[s] * w is added into acc[c] (uint64, wrapping, like the
+// reference's int64 arithmetic), the MAX region takes the max unmultiplied, and s is cleared.  canon_code is
+// idempotent, so every source is non-canonical and every destination canonical: no source changes before it is read,
+// in any order.  A slot without rows holds nothing to move.  Weighted, each slot's rows go to samples[c] first and the
+// rows left on weight code 0 without weight_carry are counted into SC_NO_WEIGHT.  Regions past `have` were not read
+// back: the result does not use them.
+static void dense_fold(sg_query* q, const FoldKey& F, uint64_t* h, size_t have, sg_result* r) {
+  const uint32_t ns = q->plan.nslots;
+  const uint64_t* cnt = h + q->off_count;
+  if (F.wradix) {
+    r->samples.assign(ns, 0);
+    for (uint32_t s = 0; s < ns; s++) {
+      if (!cnt[s]) continue;
+      if ((s / F.wstride) % F.wradix == 0 && !F.wcarry) h[SC_NO_WEIGHT] += cnt[s];
+      r->samples[canon_code(F, s)] += cnt[s];
     }
-    auto fold_array = [&](size_t off, size_t per_slot, bool is_max) {
-      if (off + (size_t)P.nslots * per_slot > have) return;  // not read back: the result does not use it
-      for (uint32_t s = 0; s < P.nslots; s++) {
-        const uint32_t code = (s / d.stride) % d.radix;
-        if (code == 0) continue;
-        uint32_t to;
-        uint64_t mul = 1;
-        if (canon && (*rtext)[code - 1].empty()) {
-          to = s - code * d.stride;  // rewritten to "": the missing group, which renders alike (DESIGN.md §7)
-        } else if (canon) {
-          if ((*canon)[code - 1] == code - 1) continue;
-          to = s - (code - 1 - (*canon)[code - 1]) * d.stride;
-        } else {
-          to = s - code * d.stride;
-          mul = wmul[code - 1];
-        }
-        uint64_t* src = h + off + (size_t)s * per_slot;
-        uint64_t* dst = h + off + (size_t)to * per_slot;
-        for (size_t k = 0; k < per_slot; k++) {
-          if (is_max)
-            dst[k] = (uint64_t)std::max((int64_t)dst[k], (int64_t)src[k]), src[k] = (uint64_t)INT64_MIN;
-          else
-            dst[k] += src[k] * mul, src[k] = 0;  // (wrapping, like the reference's int64 arithmetic)
-        }
-      }
-    };
-    for (int a = 0; a < P.naggs; a++) {
-      fold_array(q->off_hcount[(size_t)a], 1, false);
-      fold_array(q->off_sum[(size_t)a], 1, false);
-      fold_array(q->off_vmax[(size_t)a], 1, true);
-      const uint32_t nv = q->layouts[(size_t)a].nvals_total;
-      if (nv) fold_array(q->off_buckets[(size_t)a], nv, false);
-    }
-    fold_array(q->off_count, 1, false);
   }
-  return SG_OK;
+  std::vector<AccRegion> regions;
+  for (const AccRegion& R : q->regions)
+    if (R.off + (size_t)ns * R.per_row <= have) regions.push_back(R);
+  for (uint32_t s = 0; s < ns; s++) {
+    const uint32_t to = canon_code(F, s);
+    if (to == s || !cnt[s]) continue;
+    const uint64_t w = F.wradix ? (uint64_t)F.wmul[(s / F.wstride) % F.wradix] : 1u;
+    for (const AccRegion& R : regions) {
+      uint64_t* src = h + R.off + (size_t)s * R.per_row;
+      uint64_t* dst = h + R.off + (size_t)to * R.per_row;
+      for (uint32_t k = 0; k < R.per_row; k++) {
+        if (R.is_max)
+          dst[k] = (uint64_t)std::max((int64_t)dst[k], (int64_t)src[k]), src[k] = (uint64_t)INT64_MIN;
+        else
+          dst[k] += src[k] * w, src[k] = 0;
+      }
+    }
+  }
 }
 
 // A folded sparse plan's read-back: the scalars and, of every accumulator region, the rows of the L' canonical
@@ -3547,8 +3522,7 @@ static int fold_axes(sg_query* q, uint64_t* h, size_t have, sg_result* r, int64_
 static int read_canonical_rows(sg_query* q, sg_result* r) {
   sg_ctx* c = q->ctx;
   const uint32_t n = q->canon_live;
-  const size_t o_count = q->off_count;
-  const std::vector<size_t> o_sum = q->off_sum, o_hc = q->off_hcount, o_bk = q->off_buckets, o_max = q->off_vmax;
+  const std::vector<AccRegion> old = q->regions;
   int rc = layout_accumulators(q, n);
   if (rc != SG_OK) return rc;
   q->plan.nslots = n;
@@ -3562,13 +3536,7 @@ static int read_canonical_rows(sg_query* q, sg_result* r) {
     return words ? cudaMemcpyAsync(h + to, q->d_acc + from, words * 8, cudaMemcpyDeviceToHost, c->stream) : cudaSuccess;
   };
   CUDA_TRY(c, back(0, 0, SCALAR_WORDS));
-  CUDA_TRY(c, back(q->off_count, o_count, n));
-  for (size_t a = 0; a < q->layouts.size(); a++) {
-    CUDA_TRY(c, back(q->off_sum[a], o_sum[a], n));
-    CUDA_TRY(c, back(q->off_hcount[a], o_hc[a], n));
-    CUDA_TRY(c, back(q->off_buckets[a], o_bk[a], (size_t)n * q->layouts[a].nvals_total));
-    CUDA_TRY(c, back(q->off_vmax[a], o_max[a], n));
-  }
+  for (size_t i = 0; i < old.size(); i++) CUDA_TRY(c, back(q->regions[i].off, old[i].off, (size_t)n * old[i].per_row));
   CUDA_TRY(c, cudaStreamSynchronize(c->stream));
   q->d2h_bytes += (int64_t)q->acc_words * 8;
   return SG_OK;
@@ -3634,16 +3602,12 @@ int build_result(sg_query* q, sg_result** out) {
     h = (const uint64_t*)r->pin;
   }
   if (q->hashed) {
-    if (h[4] != 0) {
+    if (h[SC_TABLE_FULL] != 0) {
       c->set_err("query: the hashed slot space filled up (more distinct group keys than its table holds)");
       return SG_ERR_UNSUPPORTED;
     }
     if ((!q->repl.empty() || q->d.weight_col_slot >= 0) && !q->dfold) {
       c->set_err("query: StrReplace / weights over a hashed slot space are not in this build");
-      return SG_ERR_UNSUPPORTED;
-    }
-    if (q->dfold && h[3] != 0) {  // (fold_rows: rows left on weight code 0 without weight_carry)
-      c->set_err(NO_WEIGHT_MSG);
       return SG_ERR_UNSUPPORTED;
     }
     // slot -> key: the table itself, or for a sparse plan its id -> key array (L entries, nothing sized by the table)
@@ -3653,7 +3617,6 @@ int build_result(sg_query* q, sg_result** out) {
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     q->d2h_bytes += (int64_t)P.nslots * 4;
   }
-  int64_t w_rows = -1;  // weighted queries: matched ROWS (MatchedCount counts records, aggregate.go:117)
   if (q->dfold) {
     // folded on the device: a weighted result takes the rows per group the fold counted
     if (q->d.weight_col_slot >= 0) {
@@ -3662,24 +3625,36 @@ int build_result(sg_query* q, sg_result** out) {
         CUDA_TRY(c, cudaMemcpyAsync(r->samples.data(), q->d_samples, (size_t)P.nslots * 8, cudaMemcpyDeviceToHost, c->stream));
       CUDA_TRY(c, cudaStreamSynchronize(c->stream));
       q->d2h_bytes += (int64_t)P.nslots * 8;
-      w_rows = 0;
-      for (uint64_t n : r->samples) w_rows += (int64_t)n;
     }
   } else if (!q->repl.empty() || q->d.weight_col_slot >= 0) {
     if (q->merged && !q->repl.empty()) {
       c->set_err("query: StrReplace cannot follow a cross-GPU merge over differing dictionaries (seed them)");
       return SG_ERR_UNSUPPORTED;
     }
-    // (h is this call's own copy of the read-back)
-    const int rc = fold_axes(q, const_cast<uint64_t*>(h), have, r.get(), &w_rows);
+    FoldKey F;
+    std::vector<int64_t> wmul;
+    std::vector<uint32_t> luts;
+    const int rc = build_fold_key(q, &F, &wmul, &luts);
     if (rc != SG_OK) return rc;
+    F.wmul = wmul.data();
+    F.luts = luts.data();
+    dense_fold(q, F, const_cast<uint64_t*>(h), have, r.get());  // (h is this call's own copy of the read-back)
+  }
+  if (h[SC_NO_WEIGHT] != 0) {
+    c->set_err(NO_WEIGHT_MSG);
+    return SG_ERR_UNSUPPORTED;
+  }
+  int64_t w_rows = -1;  // weighted queries: matched ROWS (MatchedCount counts records, aggregate.go:117)
+  if (q->d.weight_col_slot >= 0) {
+    w_rows = 0;
+    for (uint64_t n : r->samples) w_rows += (int64_t)n;
   }
   r->layouts = q->layouts;
   r->hist_mode = P.hist_mode != 0;
   r->ngroups_cols = (int)q->groups.size();
   r->naggs = naggs;
-  r->matched = (int64_t)h[0];
-  r->broken = q->broken_staged + (int64_t)h[1];
+  r->matched = (int64_t)h[SC_MATCHED];
+  r->broken = q->broken_staged + (int64_t)h[SC_BROKEN];
   r->skipped = q->skipped;
   init_group(r->total, naggs);
   r->total.skey = "TOTAL";
@@ -4120,15 +4095,15 @@ int sg_query_run(sg_query* q) {
     rc = run_list(q, list);
     if (rc != SG_OK) return rc;
     const uint64_t* scal = q->h_acc.data();  // read back behind the kernel by run_list
-    if (scal[2] != 0) {
+    if (scal[SC_TIME_OVERFLOW] != 0) {
       c->set_err("query: rows fall outside the planned time axis (time_min/time_max too narrow)");
       return SG_ERR_INVALID;
     }
-    if (q->sparse && scal[5] != 0) {
-      c->set_err("query: " + std::to_string(scal[5]) + " rows' group keys were missing from the discovered sparse groups");
+    if (q->sparse && scal[SC_SPARSE_MISSING] != 0) {
+      c->set_err("query: " + std::to_string(scal[SC_SPARSE_MISSING]) + " rows' group keys were missing from the discovered sparse groups");
       return SG_ERR_STATE;
     }
-    if (scal[1] == 0) break;
+    if (scal[SC_BROKEN] == 0) break;
     std::vector<uint32_t> status(t->blocks.size());
     CUDA_TRY(c, cudaMemcpy(status.data(), q->d_block_status, status.size() * 4, cudaMemcpyDeviceToHost));
     std::vector<uint32_t> next;
@@ -4371,13 +4346,12 @@ static int remap_to_union(sg_query* q) {
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     q->d2h_bytes += (int64_t)q->acc_words * 8;
     const size_t o_count = q->off_count;
-    const std::vector<size_t> o_hc = q->off_hcount, o_sum = q->off_sum, o_vmax = q->off_vmax, o_bk = q->off_buckets;
+    const std::vector<AccRegion> old = q->regions;
     rc = layout_accumulators(q, new_slots);
     if (rc != SG_OK) return rc;
     std::vector<uint64_t> h_new(q->acc_words, 0);
     for (size_t w = q->sum_words; w < q->acc_words; w++) h_new[w] = (uint64_t)INT64_MIN;
     for (size_t w = 0; w < SCALAR_WORDS; w++) h_new[w] = h_old[w];
-    const int naggs = P.naggs;
     for (uint32_t s = 0; s < old_slots; s++) {
       if (h_old[o_count + s] == 0) continue;
       uint64_t ns = 0;
@@ -4386,14 +4360,9 @@ static int remap_to_union(sg_query* q) {
         uint32_t code = (s / od.stride) % od.radix;
         ns += (uint64_t)remap[di][code] * ndims[di].stride;
       }
-      h_new[q->off_count + ns] = h_old[o_count + s];
-      for (int a = 0; a < naggs; a++) {
-        h_new[q->off_hcount[(size_t)a] + ns] = h_old[o_hc[(size_t)a] + s];
-        h_new[q->off_sum[(size_t)a] + ns] = h_old[o_sum[(size_t)a] + s];
-        h_new[q->off_vmax[(size_t)a] + ns] = h_old[o_vmax[(size_t)a] + s];
-        const uint32_t nv = q->layouts[(size_t)a].nvals_total;
-        if (nv)
-          memcpy(&h_new[q->off_buckets[(size_t)a] + (size_t)ns * nv], &h_old[o_bk[(size_t)a] + (size_t)s * nv], (size_t)nv * 8);
+      for (size_t i = 0; i < old.size(); i++) {
+        const size_t w = old[i].per_row;
+        memcpy(&h_new[q->regions[i].off + (size_t)ns * w], &h_old[old[i].off + (size_t)s * w], w * 8);
       }
     }
     pool_release(c, q->d_acc);
@@ -4462,7 +4431,7 @@ int sg_query_allreduce(sg_query* q) {
       return SG_ERR_CUDA;
     }
     CUDA_TRY(c, pool_alloc(c, (void**)&d_all, aw * 8 * nr));
-    uint64_t* hdr = (uint64_t*)hp;
+    uint64_t* hdr = (uint64_t*)hp;  // the merge header: words SC_MERGE.. of the scalars
     hdr[0] = (uint64_t)q->broken_staged;
     hdr[1] = (uint64_t)q->skipped;
     hdr[2] = (uint64_t)q->rows_scanned;
@@ -4470,7 +4439,7 @@ int sg_query_allreduce(sg_query* q) {
     hdr[4] = sig;
     hdr[5] = (uint64_t)axes_size;
     hdr[6] = hdr[7] = 0;
-    CUDA_TRY(c, cudaMemcpyAsync(q->d_acc + 8, hdr, 64, cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(c, cudaMemcpyAsync(q->d_acc + SC_MERGE, hdr, 64, cudaMemcpyHostToDevice, c->stream));
     ncclResult_t r = g_nccl.AllGather(q->d_acc, d_all, aw * 8, ncclUint8, c->comm, c->stream);
     if (r != 0) return nccl_fail(c, "ncclAllGather", r);
     uint64_t* all = (uint64_t*)(hp + 64);
@@ -4479,11 +4448,11 @@ int sg_query_allreduce(sg_query* q) {
     pool_release(c, d_all);
     q->d2h_bytes += (int64_t)(aw * 8 * nr);
     bool agree = true;
-    for (size_t k = 0; k < nr; k++) agree = agree && all[k * aw + 12] == sig && all[k * aw + 13] == (uint64_t)axes_size;
+    for (size_t k = 0; k < nr; k++) agree = agree && all[k * aw + SC_MERGE_AXES] == sig && all[k * aw + SC_MERGE_AXES + 1] == (uint64_t)axes_size;
     // the counters are job totals on either path
     uint64_t tot[4] = {0, 0, 0, 0};
     for (size_t k = 0; k < nr; k++)
-      for (int j = 0; j < 4; j++) tot[j] += all[k * aw + 8 + (size_t)j];
+      for (int j = 0; j < 4; j++) tot[j] += all[k * aw + SC_MERGE + (size_t)j];
     if (agree) {
       q->h_acc.assign(aw, 0);
       uint64_t* h = q->h_acc.data();
@@ -4505,7 +4474,7 @@ int sg_query_allreduce(sg_query* q) {
       return SG_OK;
     }
     // differing axes: every rank sees that in the same gathered data and takes the exchange path
-    CUDA_TRY(c, cudaMemsetAsync(q->d_acc + 8, 0, 64, c->stream));
+    CUDA_TRY(c, cudaMemsetAsync(q->d_acc + SC_MERGE, 0, 64, c->stream));
   }
   // ---- larger plans: element-wise all-reduces (sums: scalars, count, hcount, sum, buckets; max: vmax) --------
   const uint64_t sig = axes_signature(q, nullptr);
@@ -4544,7 +4513,7 @@ int sg_query_allreduce(sg_query* q) {
       return SG_ERR_CUDA;
     }
     CUDA_TRY(c, pool_alloc(c, (void**)&d_merged, q->acc_words * 8));
-    uint64_t* hc = (uint64_t*)hp;
+    uint64_t* hc = (uint64_t*)hp;  // the merge header: words SC_MERGE.. of the scalars
     hc[0] = (uint64_t)q->broken_staged;
     hc[1] = (uint64_t)q->skipped;
     hc[2] = (uint64_t)q->rows_scanned;
@@ -4568,13 +4537,13 @@ int sg_query_allreduce(sg_query* q) {
         to_pin = true;
       }
     }
-    cudaError_t ce = cudaMemcpyAsync(q->d_acc + 8, hc, 64, cudaMemcpyHostToDevice, c->stream);
+    cudaError_t ce = cudaMemcpyAsync(q->d_acc + SC_MERGE, hc, 64, cudaMemcpyHostToDevice, c->stream);
     if (ce == cudaSuccess) {
       rc = ar(q->d_acc, d_merged, q->sum_words, ncclUint64, ncclSum);
       if (rc == SG_OK && q->acc_words > q->sum_words)
         rc = ar(q->d_acc + q->sum_words, d_merged + q->sum_words, q->acc_words - q->sum_words, ncclInt64, ncclMax);
     }
-    if (ce == cudaSuccess && rc == SG_OK) ce = cudaMemsetAsync(q->d_acc + 8, 0, 64, c->stream);  // own copy as it was
+    if (ce == cudaSuccess && rc == SG_OK) ce = cudaMemsetAsync(q->d_acc + SC_MERGE, 0, 64, c->stream);  // own copy as it was
     if (ce == cudaSuccess && rc == SG_OK)
       ce = cudaMemcpyAsync(hm, d_merged, whole ? q->acc_words * 8 : 128, cudaMemcpyDeviceToHost, c->stream);
     if (ce == cudaSuccess && rc == SG_OK) ce = cudaStreamSynchronize(c->stream);
@@ -4584,7 +4553,7 @@ int sg_query_allreduce(sg_query* q) {
       c->set_err(std::string("merge: ") + cudaGetErrorString(ce));
       return SG_ERR_CUDA;
     }
-    const uint64_t* m = hm + 8;
+    const uint64_t* m = hm + SC_MERGE;
     const bool agree = m[4] == n * sa && m[5] == n * sa * sa && m[6] == n * sb && m[7] == n * sb * sb;
     q->broken_staged = (int64_t)m[0];
     q->skipped = (int64_t)m[1];
@@ -4592,7 +4561,7 @@ int sg_query_allreduce(sg_query* q) {
     q->blocks_scanned = (int64_t)m[3];
     if (agree) {
       // the merged copy becomes the query's accumulator array (the plan's device pointers name q->d_acc)
-      ce = cudaMemsetAsync(d_merged + 8, 0, 64, c->stream);
+      ce = cudaMemsetAsync(d_merged + SC_MERGE, 0, 64, c->stream);
       if (ce == cudaSuccess) ce = cudaMemcpyAsync(q->d_acc, d_merged, q->acc_words * 8, cudaMemcpyDeviceToDevice, c->stream);
       if (ce == cudaSuccess && !whole) ce = cudaStreamSynchronize(c->stream);
       pool_release(c, d_merged);  // (stream-ordered pool: reuse waits for the copy queued above)
@@ -4601,9 +4570,9 @@ int sg_query_allreduce(sg_query* q) {
         return SG_ERR_CUDA;
       }
       if (whole) {
-        for (int k = 8; k < 16; k++) hm[k] = 0;
+        for (int k = SC_MERGE; k < SCALAR_WORDS; k++) hm[k] = 0;
         if (to_pin) {
-          q->h_acc.assign(hm, hm + 8);
+          q->h_acc.assign(hm, hm + SC_MERGE);
           q->h_pin_valid = true;
         } else {
           q->h_acc.assign(hm, hm + q->acc_words);

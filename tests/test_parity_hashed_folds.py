@@ -1,7 +1,7 @@
 """Weighted and StrReplace group-bys over hashed and sparse group keys, folded on the device
 (sg_query_set_hashed_folds, engine.FLAGS.HASHED_FOLDS).  Every folded result is checked bit for bit against the
 row-level reference tests/rowref.py and, where the same query runs on a dense plan (folded on the host by
-fold_axes), against that run's complete listing.  Tables: tests/edges.py (families W and R),
+dense_fold), against that run's complete listing.  Tables: tests/edges.py (families W and R),
 tests/test_parity_weight_carry.py and tables built here in the shape of tests/family_sparse.py."""
 import ctypes as C
 import re
