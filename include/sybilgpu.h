@@ -281,7 +281,9 @@ int64_t sg_table_h2d_bytes(sg_table* t);     /* bytes copied host->device while 
 sg_query* sg_query_begin(sg_ctx* ctx, sg_table* t, const sg_query_desc* desc);
 void sg_query_free(sg_query* q);
 /* host-evaluated regex for filter #filter_index (filter.go:215-237): bitset over the
- * GLOBAL string ids of that column, nbits = sg_table_dict_size at call time */
+ * GLOBAL string ids of that column, nbits = sg_table_dict_size at call time.  Blocks staged
+ * later (sg_table_add_block, sg_query_submit_block) may add strings; planning then refuses the
+ * query with SG_ERR_STATE until the bitset is set again over the grown dictionary. */
 int sg_query_set_str_lut(sg_query* q, int32_t filter_index, const uint32_t* bits, int64_t nbits);
 /* StrReplace (FLAGS.STR_REPLACE "col:pattern:replacement", table_query.go:34-50): the reference rewrites a str
  * column's string table with regexp.ReplaceAllString while it unpacks a block (column_store_io.go:515-549), so

@@ -2120,6 +2120,14 @@ int make_plan(sg_query* q, const std::vector<uint32_t>& list) {
           c->set_err("query: regex filter without sg_query_set_str_lut");
           return SG_ERR_STATE;
         }
+        // strings interned after the bitset was built have no bit: the kernel would read them as "no match"
+        // (RE drops their rows, NRE keeps them), so a dictionary that grew since needs the bitset set again
+        if (q->lut_bits[(size_t)i] < (int64_t)t->sdict[(size_t)f.col_slot].strs.size()) {
+          c->set_err("query: filter " + std::to_string(i) + ": the regex bitset covers " +
+                     std::to_string(q->lut_bits[(size_t)i]) + " strings, the column's dictionary now holds " +
+                     std::to_string(t->sdict[(size_t)f.col_slot].strs.size()) + " (sg_query_set_str_lut again)");
+          return SG_ERR_STATE;
+        }
         kf.lut = q->d_luts[(size_t)i];
         kf.lut_bits = q->lut_bits[(size_t)i];
       } else {

@@ -534,20 +534,29 @@ class PreparedQuery:
                     offs[1:] = np.cumsum([len(x) for x in strs])
                 buf = np.frombuffer(blob if blob else b"\0", dtype=np.uint8).copy()
                 ctx.check(lib.sg_query_set_str_replace(self.q, table.KeyTable[name], buf.ctypes.data, offs.ctypes.data, len(strs)))
+            # regex filters of columns without StrReplace: {filter index: (filter, strings the bitset covers)}; Run
+            # sets the bitset again when blocks staged since brought new strings
+            self._regex = {}
             for i, f in enumerate(qs.Filters):
                 if isinstance(f, StrFilter) and (f.regex is not None or f.Field in repl):
-                    # the host evaluates the regexp once per distinct string (filter.go:215-237)
                     strs = rewritten[f.Field] if f.Field in repl else table.dict_strings(f.Field)
-                    bits = np.zeros((len(strs) + 31) // 32 + 1, np.uint32)
-                    lit = f.Value if isinstance(f.Value, bytes) else f.Value.encode()
-                    for gid, s in enumerate(strs):
-                        hit = f.regex.search(s.decode("utf-8", "replace")) if f.regex is not None else s == lit
-                        if hit:
-                            bits[gid >> 5] |= np.uint32(1 << (gid & 31))
-                    ctx.check(lib.sg_query_set_str_lut(self.q, i, bits.ctypes.data, len(strs)))
+                    self._set_lut(i, f, strs)
+                    if f.Field not in repl:  # (a grown StrReplace column is refused: sg_query_set_str_replace)
+                        self._regex[i] = (f, len(strs))
         except Exception:
             self.Close()
             raise
+
+    def _set_lut(self, i, f, strs):
+        """The match bitset of filter i over the column's global string ids: the host evaluates the regexp once per
+        distinct string (filter.go:215-237)."""
+        bits = np.zeros((len(strs) + 31) // 32 + 1, np.uint32)
+        lit = f.Value if isinstance(f.Value, bytes) else f.Value.encode()
+        for gid, s in enumerate(strs):
+            hit = f.regex.search(s.decode("utf-8", "replace")) if f.regex is not None else s == lit
+            if hit:
+                bits[gid >> 5] |= np.uint32(1 << (gid & 31))
+        self.table.ctx.check(self.table.lib.sg_query_set_str_lut(self.q, i, bits.ctypes.data, len(strs)))
 
     def Run(self, qs, allreduce=False, fill_later=False):
         """One pass of the hot path; fills qs like LoadAndQueryRecords.  The result object is freed before
@@ -557,6 +566,11 @@ class PreparedQuery:
         of the timed region this way."""
         t = self.table
         lib, ctx = t.lib, t.ctx
+        for i, (f, n) in self._regex.items():
+            if lib.sg_table_dict_size(t.h, f.FieldId) != n:
+                strs = t.dict_strings(f.Field)
+                self._set_lut(i, f, strs)
+                self._regex[i] = (f, len(strs))
         ctx.check(lib.sg_query_run(self.q))
         if allreduce:
             ctx.check(lib.sg_query_allreduce(self.q))

@@ -55,25 +55,19 @@ def _no_oracle(q):
     return q
 
 
-def _no_rowref(q):
-    q.rowref = False  # regular expressions: tests/rowref.py restates eq / neq only; the oracle checks these
-    return q
-
-
 def _queries(s):
     q = edges._q
     return [
         # count mode (s2 and k are partial): int and str filters of every op, first and second group with aliases
         q(s, int_filters=[("b255", "gt", 100), ("b254", "lt", 120)], str_filters=[("s2", "neq", "x3")],
           groups=["s", "k"], aggs=["v"], op="hist", expect=[r"fail_mode=0 ", r"codes=5\b"]),
-        _no_rowref(q(s, int_filters=[("k", "eq", 5), ("b2", "neq", 0)], str_filters=[("s2", "re", "^x1")],
-                     groups=["k", "s2"], aggs=["v"], op="avg", expect=[r"codes=5\b"])),
+        q(s, int_filters=[("k", "eq", 5), ("b2", "neq", 0)], str_filters=[("s2", "re", "^x1")], groups=["k", "s2"],
+          aggs=["v"], op="avg", expect=[r"codes=5\b"]),
         # fail mode over full code columns, next to a 1,000-bin push-down filter and value arrays (the bench shape)
         q(s, int_filters=[("f", "gt", 100), ("v", "lt", 900000)], str_filters=[("s", "neq", "s3")], groups=["s", "b2"],
           aggs=["v"], op="hist", expect=[r"fail_mode=1 ", r"codes=3\b"]),
-        _no_rowref(q(s, int_filters=[("b255", "eq", 3), ("b254", "neq", 0), ("b1", "lt", 8)],
-                     str_filters=[("s", "nre", "^s1")], groups=["b254"], aggs=["v"], op="avg",
-                     expect=[r"fail_mode=1 ", r"codes=5\b"])),
+        q(s, int_filters=[("b255", "eq", 3), ("b254", "neq", 0), ("b1", "lt", 8)], str_filters=[("s", "nre", "^s1")],
+          groups=["b254"], aggs=["v"], op="avg", expect=[r"fail_mode=1 ", r"codes=5\b"]),
         q(s, int_filters=[("b255", "lt", 200), ("b1", "eq", 7)], str_filters=[("s", "eq", "s4")], groups=["b255"],
           aggs=["v"], op="avg", expect=[r"fail_mode=1 ", r"codes=4\b"]),
         # 1 / 2 / 254 / 255 bins read through codes, 256 through ids
@@ -138,13 +132,12 @@ def _run(forms, monkeypatch, capfd, variant, env=()):
         if "SG_FORCE_HASHED_SLOTS" in env and (q.weight_col or q.str_replace):
             continue  # (weights and StrReplace over a hashed slot space are refused)
         if i not in _REF:  # (neither depends on the array form, the build or the switches)
-            _REF[i] = rowref.run(spec, rows, valid, q) if getattr(q, "rowref", True) else None
+            _REF[i] = rowref.run(spec, rows, valid, q)
             _ORC[i] = run_oracle(spec, q) if getattr(q, "oracle", True) else None
         where = (forms, variant, env, i)
         g, trace = _gpu(spec, q, monkeypatch, capfd, False)
         assert g.BrokenBlocks == 0, where
-        if _REF[i] is not None:
-            rowref.check(_REF[i], g, q, where=where)
+        rowref.check(_REF[i], g, q, where=where)
         if _ORC[i] is not None:
             compare(g, _ORC[i], q, mean=_mean_comparable)
         for pat in q.expect:

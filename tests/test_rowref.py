@@ -4,11 +4,11 @@ the scan kernel branches, so a misreading the oracle shares with the kernel cann
 import numpy as np
 import pytest
 
-from tests import edges, rowref
+from tests import edges, family_p, rowref
 from tests.test_oracle_vs_py import py_query
 from tests.util import run_oracle
 
-TABLES = edges.all_tables()
+TABLES = edges.all_tables() + [(name, build()) for name, build in family_p.P_TABLES.items()]
 SMALL = 30000  # rows: pyoracle's per-row loops are run on tables up to this size
 
 
@@ -159,3 +159,83 @@ def test_rowref_rules():
     assert rowref.basic_layout(0, 10 ** 6, 7) == (7, 1002)
     subs = rowref.multi_layout(0, 1 << 20)
     assert subs[0] == ((1 << 19), 1 << 20) and subs[-1][0] == 0 and len(subs) == 12
+    # StrFilter re / nre (filter.go:199-250): MatchString is an unanchored search on the decoded string
+    assert rowref._str_pass("re", "", "^$") and not rowref._str_pass("nre", "", "^$")
+    assert rowref._str_pass("re", "", "") and not rowref._str_pass("re", "", ".")
+    assert rowref._str_pass("re", "s12", "^s1") and not rowref._str_pass("re", "xs1", "^s1")
+    assert rowref._str_pass("re", "s21", "1$") and not rowref._str_pass("re", "s12", "1$")
+    assert rowref._str_pass("re", "s33", "^(s3|s33)$") and not rowref._str_pass("re", "s333", "^(s3|s33)$")
+    # a row without the column fails re and nre alike, whatever the pattern
+    from tests.util import STR, Q, Spec
+    s = Spec([("g", STR)])
+    cols, va = {"g": np.array(["", "s1", "x", "s1"])}, {"g": np.array([True, True, True, False])}
+    s.add_rows(cols, va)
+    rows, valid = [(cols, None, 5000)], [va]
+    for op, pat, want in (("re", "^$", 1), ("nre", "^$", 2), ("re", "", 3), ("nre", "", 0), ("nre", "zz", 3),
+                          ("re", "1$", 1)):
+        q = Q(s, str_filters=[("g", op, pat)], groups=["g"])
+        assert rowref.run(s, rows, valid, q).MatchedCount == want, (op, pat)
+
+
+def _global_dict(spec, name):
+    """A str column's global dictionary as staging builds it: each block's string table in order, then "" (interned
+    for every block's str column, sg_table_add_block)."""
+    d = {}
+    for b in spec.blocks:
+        for c in b.cols:
+            if c.col_slot == spec.KeyTable[name]:
+                for s in c.string_table + [b""]:
+                    d.setdefault(s, len(d))
+    return list(d)
+
+
+def test_p_tables_hold_their_forms():
+    """Family P's columns are in the forms the family claims: a partial bucket column, full code columns, full
+    bucket columns of 256 to 1,025 bins straddling 1,024-entry tiles, value arrays on the 32-bit path with int16 and
+    int32 deltas on a base near 2^32, value arrays with negatives and values past 2^32, value arrays shorter than
+    their block, a column absent from some blocks, and str dictionaries of 33 and 65 strings whose last string is the
+    only one its pattern matches."""
+    import re
+    from sybil_b200 import _ffi as F
+    U32 = family_p.U32
+    spec, rows, valid, qs = family_p.family_p_sweep("narrow")
+    gspec = dict(TABLES)["P-geom"][0]
+
+    def cols(sp, name, enc=None):
+        out = [(b, c) for b in sp.blocks for c in b.cols if c.col_slot == sp.KeyTable[name]]
+        return [(b, c) for b, c in out if enc is None or c.encoding == enc]
+
+    def nlisted(c):
+        return len(c.record_ids)
+
+    bucket = F.SG_ENC_BUCKET
+    values = F.SG_ENC_VALUES
+    assert any(nlisted(c) < b.num_records for b, c in cols(spec, "bp", bucket))
+    for name in ["bc", "sc"] + family_p.P_CODES:
+        bc = cols(spec, name, bucket)
+        assert bc and all(nlisted(c) == b.num_records and len(c.bin_values) <= 255 for b, c in bc), name
+    for sp in (spec, gspec):
+        bd = [(b, c) for b, c in cols(sp, "bd", bucket) if b.num_records >= 1024]
+        assert bd and all(nlisted(c) == b.num_records and 256 <= len(c.bin_values) <= 1025 for b, c in bd)
+    big = [c for b, c in cols(gspec, "bd", bucket) if b.num_records >= 65535]
+    assert len(big) == 2 and all(any(int(o0) >> 10 != (int(o1) - 1) >> 10 for o0, o1 in
+                                     zip(c.bin_offsets[:-1], c.bin_offsets[1:])) for c in big)
+    assert any(len(c.bin_values) > 255 for b, c in cols(spec, "sm", bucket))
+    v32 = cols(spec, "v32", values)
+    assert {np.asarray(c.values_i64).dtype for b, c in v32 if b.num_records > 1} == {np.dtype(np.int16),
+                                                                                     np.dtype(np.int32)}
+    assert all(U32 - (1 << 24) <= c.value_base < U32 for b, c in v32 if b.num_records > 1)
+    v = [int(x) for cl, _, _ in rows for x in cl["v32"]]
+    assert min(v) >= 0 and max(v) == U32 - 1
+    v = set(int(x) for cl, _, _ in rows for x in cl["v64"])
+    assert min(v) < 0 and max(v) > U32
+    for name in ("vs", "sv"):
+        short = cols(spec, name, values)
+        arr = (lambda c: c.values_i64) if name == "vs" else (lambda c: c.values_i32)
+        assert any(len(arr(c)) < b.num_records for b, c in short), name
+    assert 0 < len(cols(spec, "ab")) < len(spec.blocks)
+    for name, size, last, pat in (("d33", 33, "pz", "^p"), ("d65", 65, "qz", "^q")):
+        d = _global_dict(spec, name)
+        assert len(d) == size and d[-1] == last.encode(), (name, len(d), d[-3:])
+        assert [s for s in d if re.search(pat, s.decode())] == [last.encode()], name
+        assert any(last in set(cl[name][va[name]]) for (cl, _, _), va in zip(rows, valid) if name in va)
