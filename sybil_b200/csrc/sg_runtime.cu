@@ -1350,6 +1350,39 @@ struct ResultGroup {
   }
 };
 
+// Words [0, words) of the accumulator array on the host (read_acc fills it): in a pinned buffer of the context's
+// pool, which goes back to the pool with the object, or in a vector.  Move-only: a result takes over its query's.
+struct HostAcc {
+  sg_ctx* c = nullptr;
+  char* pin = nullptr;
+  size_t pin_bytes = 0;
+  std::vector<uint64_t> vec;
+  size_t words = 0;  // 0: no copy (a pinned buffer may still be held for the next read)
+  HostAcc() = default;
+  HostAcc& operator=(HostAcc&& o) noexcept {
+    unpin();
+    c = o.c;
+    pin = std::exchange(o.pin, nullptr);
+    pin_bytes = std::exchange(o.pin_bytes, 0);
+    vec = std::move(o.vec);
+    words = std::exchange(o.words, 0);
+    return *this;
+  }
+  ~HostAcc() { unpin(); }
+  uint64_t* data() { return pin ? (uint64_t*)pin : vec.data(); }
+  void unpin() {
+    if (pin) c->pin_put(pin, pin_bytes);
+    pin = nullptr;
+  }
+  // a copy made on the host: n words, zeroed, in the vector
+  uint64_t* host(size_t n) {
+    unpin();
+    vec.assign(n, 0);
+    words = n;
+    return vec.data();
+  }
+};
+
 }  // namespace
 
 struct sg_result {
@@ -1368,12 +1401,7 @@ struct sg_result {
   // lists the (limit) slots in sorted order and a ResultGroup is built the first time it is asked for — a
   // 1M-group result no longer renders and sorts a million keys on the host per query
   bool lazy = false;
-  std::vector<uint64_t> acc;  // accumulator words [0, acc_have): small results
-  char* pin = nullptr;        // ... large results: a pinned buffer of the context's pool
-  size_t pin_bytes = 0;
-  const uint64_t* accp = nullptr;
-  size_t acc_have = 0;
-  ~sg_result();
+  HostAcc acc;
   std::vector<uint32_t> order;
   int64_t ngroups_total = 0;
   std::unordered_map<int64_t, std::unique_ptr<ResultGroup>> cache;
@@ -1469,14 +1497,10 @@ struct sg_query {
   uint32_t canon_live = 0;         // sparse: canonical entries, which hold ids 0..canon_live-1
   double insert_ms = 0, fold_ms = 0;
   cudaEvent_t ev2 = nullptr, ev3 = nullptr;
-  // accumulators as read back right behind the kernel (small plans): spares build_result a blocking copy
-  std::vector<uint64_t> h_acc;
-  bool h_acc_valid = false;
-  // ... larger ones (tens of KB to 4 MiB: a C3-shaped result is 0.94 MB) land in a pinned buffer of the context's
-  // pool that the result then OWNS — no copy out of the scratch area (that copy cost as much as the D2H itself)
-  char* h_pin = nullptr;
-  size_t h_pin_bytes = 0;
-  bool h_pin_valid = false;
+  // the whole accumulator array as read back right behind the last launch or merge (arrays up to 4 MiB: a C3-shaped
+  // one is 0.94 MB): spares build_result a blocking copy, and its result takes the copy over
+  HostAcc acc;
+  uint64_t scal[SC_MERGE] = {};  // the scalars of the last launch (run_list)
   uint64_t axes_sig = 0, axes_sig_version = 0;  // axes_signature(): valid for table version axes_sig_version - 1
   size_t axes_size = 0;
   // multi-GPU: aggregations whose hist Count the kernel skipped on THIS rank (== Count here); the count array is
@@ -1493,11 +1517,49 @@ struct sg_query {
   std::map<int, Replace> repl;
 };
 
-sg_result::~sg_result() {
-  if (pin && q) q->ctx->pin_put(pin, pin_bytes);
-}
-
 namespace {
+
+// Reads words [0, words) of the accumulator array into h: the one place that picks pinned or pageable storage for it.
+// An array of pin_from bytes or more lands in a pinned buffer of the context's pool (h's own when large enough) that
+// h then holds, so nothing is copied out afterwards (that copy cost as much as the read itself).  A smaller one, or
+// one no pinned buffer can be had for, lands in `stage` and is copied to a vector; without a stage the pinned buffer
+// is required (a pageable destination is staged by the driver at a fraction of the PCIe rate).  `stage` is pinned
+// scratch (sg_ctx::scratch) that copies queued earlier on c->stream may still read, and that the next query reuses:
+// the copies into it queue behind those, and it is read only after the stream is synchronised.  copy(dst) queues the
+// device-to-host copies on c->stream.
+template <class Copy>
+int read_acc(sg_query* q, HostAcc& h, size_t words, size_t pin_from, char* stage, Copy copy) {
+  sg_ctx* c = q->ctx;
+  const size_t bytes = words * 8;
+  h.c = c;
+  h.words = 0;
+  char* dst = nullptr;
+  if (bytes >= pin_from) {
+    if (h.pin && h.pin_bytes < bytes) h.unpin();
+    if (!h.pin) h.pin = c->pin_get(bytes, &h.pin_bytes);
+    dst = h.pin;
+  }
+  if (!dst) dst = stage;
+  if (!dst) {
+    c->set_err("cudaHostAlloc (result buffer) failed");
+    return SG_ERR_CUDA;
+  }
+  CUDA_TRY(c, copy((uint64_t*)dst));
+  CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+  if (dst == stage) {
+    h.unpin();
+    h.vec.assign((const uint64_t*)stage, (const uint64_t*)stage + words);
+  }
+  h.words = words;
+  return SG_OK;
+}
+int read_acc(sg_query* q, HostAcc& h, const uint64_t* src, size_t words, size_t pin_from, char* stage) {
+  return read_acc(q, h, words, pin_from, stage, [&](uint64_t* dst) {
+    return cudaMemcpyAsync(dst, src, words * 8, cudaMemcpyDeviceToHost, q->ctx->stream);
+  });
+}
+// whole arrays from this size on are read into a pinned buffer of the pool rather than through the scratch area
+constexpr size_t PIN_WHOLE_FROM = (size_t)32 << 10;
 
 void free_device(sg_query* q) {
   sg_ctx* c = q->ctx;
@@ -2754,25 +2816,15 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list, bool discover = fal
     rc = device_fold(q, discover);
     if (rc != SG_OK) return rc;
   }
-  const bool to_pin = acc_back == q->acc_words * 8 && acc_back >= ((size_t)32 << 10);
-  q->h_pin_valid = false;
-  if (to_pin) {
-    if (q->h_pin && q->h_pin_bytes < acc_back) {
-      c->pin_put(q->h_pin, q->h_pin_bytes);
-      q->h_pin = nullptr;
-    }
-    if (!q->h_pin) q->h_pin = c->pin_get(acc_back, &q->h_pin_bytes);
-  }
-  char* const back = to_pin && q->h_pin ? q->h_pin : hp + off_acc;
-  CUDA_TRY(c, cudaMemcpyAsync(back, discover ? q->d_disc : q->d_acc, acc_back, cudaMemcpyDeviceToHost, c->stream));
-  CUDA_TRY(c, cudaStreamSynchronize(c->stream));
-  if (back == q->h_pin) {
-    q->h_acc.assign((const uint64_t*)back, (const uint64_t*)back + SC_MERGE);  // the scalars (sg_query_run reads them)
-    q->h_acc_valid = false;
-    q->h_pin_valid = true;
+  if (acc_back == q->acc_words * 8) {
+    rc = read_acc(q, q->acc, q->d_acc, q->acc_words, PIN_WHOLE_FROM, hp + off_acc);
+    if (rc != SG_OK) return rc;
+    memcpy(q->scal, q->acc.data(), sizeof(q->scal));
   } else {
-    q->h_acc.assign((const uint64_t*)back, (const uint64_t*)(back + acc_back));
-    q->h_acc_valid = acc_back == q->acc_words * 8;
+    q->acc.words = 0;
+    CUDA_TRY(c, cudaMemcpyAsync(hp + off_acc, discover ? q->d_disc : q->d_acc, acc_back, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    memcpy(q->scal, hp + off_acc, sizeof(q->scal));
   }
   q->d2h_bytes += (int64_t)acc_back;
   float ms = 0;
@@ -2789,7 +2841,7 @@ int run_list(sg_query* q, const std::vector<uint32_t>& list, bool discover = fal
     q->fold_ms = fms;
     if (!discover && getenv("SG_PLAN_TRACE"))
       fprintf(stderr, "sg_fold: entries=%llu canon=%llu insert_ms=%.4f fold_ms=%.4f\n",
-              (unsigned long long)q->h_acc[SC_FOLD_ENTRIES], (unsigned long long)q->h_acc[SC_FOLD_CANON], q->insert_ms,
+              (unsigned long long)q->scal[SC_FOLD_ENTRIES], (unsigned long long)q->scal[SC_FOLD_CANON], q->insert_ms,
               q->fold_ms);
   }
   if (d_dbg) {
@@ -3039,7 +3091,7 @@ int discover_groups(sg_query* q, const std::vector<uint32_t>& list) {
   int rc = run_list(q, list, true);
   P.scalars = acc_scalars;
   if (rc != SG_OK) return rc;
-  const uint64_t* scal = q->h_acc.data();
+  const uint64_t* scal = q->scal;
   if (scal[SC_TIME_OVERFLOW] != 0) {
     c->set_err("query: rows fall outside the planned time axis (time_min/time_max too narrow)");
     return SG_ERR_INVALID;
@@ -3123,9 +3175,10 @@ std::string render_key(const sg_query* q, const std::vector<uint64_t>& key) {
   return s;
 }
 
-void merge_group(ResultGroup& into, const ResultGroup& g, int naggs, const std::vector<HistLayout>& L, bool with_hists) {
+// g's Count, hist Counts, sums, maxima and bucket counters added into `into`; an aggregation whose hist Count is 0 in
+// g adds nothing
+void merge_group(ResultGroup& into, const ResultGroup& g, int naggs, const std::vector<HistLayout>& L) {
   into.count += g.count;
-  if (!with_hists) return;
   for (int a = 0; a < naggs; a++) {
     if (g.hc(a) == 0) continue;
     into.hc(a) += g.hc(a);
@@ -3254,6 +3307,64 @@ static std::string slot_key(const sg_query* q, uint32_t s) {
   group_key(q, s, g, nullptr);
   return std::move(g.skey);
 }
+
+// The order of the slots of a result without a time axis, as sort_groups orders rendered keys: order value
+// descending, ties by the rendered GroupByKey ascending.  That is lexicographic over the axes' field ranks when they
+// are `plain`; otherwise tied entries compare their rendered keys (`keys` by Ent::row when the caller rendered them
+// once, slot_key otherwise).
+struct GroupOrder {
+  struct Ent {
+    double v;
+    uint64_t tie;
+    uint32_t slot;
+    uint32_t row;  // the device top-K: the candidate's row
+  };
+  const sg_query* q;
+  std::vector<std::vector<uint32_t>> scratch;
+  std::vector<const std::vector<uint32_t>*> ranks;
+  bool plain = true;
+  std::vector<std::string> keys;
+  // ranked false: the groups stay in slot order (OrderBy ""), nothing to rank
+  GroupOrder(sg_query* q, bool ranked) : q(q), scratch(q->dims.size()), ranks(q->dims.size(), nullptr) {
+    if (ranked)
+      for (size_t di = 0; di < q->dims.size(); di++) ranks[di] = &axis_ranks(q, di, scratch[di], &plain);
+  }
+  // the tie rank of a code (the missing value's digit 0 first on every axis)
+  uint64_t tie(uint32_t code) const {
+    uint64_t t = 0;
+    for (size_t di = 0; di < q->dims.size(); di++) {
+      const GroupDim& d = q->dims[di];
+      const uint32_t digit = (code / d.stride) % d.radix;
+      t = t * d.radix + (digit ? (uint64_t)(*ranks[di])[digit - 1] + 1u : 0u);
+    }
+    return t;
+  }
+  bool before(const Ent& a, const Ent& b) const {
+    if (a.v != b.v) return a.v > b.v;
+    if (plain) return a.tie < b.tie;
+    return keys.empty() ? slot_key(q, a.slot) < slot_key(q, b.slot) : keys[a.row] < keys[b.row];
+  }
+};
+
+// A result of q without groups: the header every result of the query carries and an empty Cumulative.  scal: the
+// scalars of the accumulators it is built from, for the broken blocks; a time slice (nullptr) carries no block
+// counters and its Cumulative no key.
+static std::unique_ptr<sg_result> new_result(sg_query* q, bool hist_mode, const uint64_t* scal) {
+  std::unique_ptr<sg_result> r(new sg_result());
+  r->q = q;
+  r->layouts = q->layouts;
+  r->hist_mode = hist_mode;
+  r->ngroups_cols = (int)q->groups.size();
+  r->naggs = q->plan.naggs;
+  init_group(r->total, r->naggs);
+  if (scal) {
+    r->broken = q->broken_staged + (int64_t)scal[SC_BROKEN];
+    r->skipped = q->skipped;
+    r->total.skey = "TOTAL";
+    for (int i = 1; i < (int)q->groups.size(); i++) r->total.skey += "\t";
+  }
+  return r;
+}
 static void make_group(const sg_query* q, const uint64_t* h, uint32_t s, ResultGroup& g, int64_t* tbucket,
                        const std::vector<uint64_t>* samples = nullptr) {
   const Plan& P = q->plan;
@@ -3309,7 +3420,10 @@ static int build_result_topk(sg_query* q, sg_result** out, bool* fell_back) {
   if (!q->repl.empty() || q->d.weight_col_slot >= 0) return 1;  // StrReplace / weights fold slots on the host first
   if (q->hashed) return 1;                                       // keys come from the table read-back (build_result)
   if (limit <= 0 || limit > 65536 || ob == SG_ORDER_NONE || q->d.order_asc) return 1;
-  if (P.nslots < (1u << 17) || q->h_acc_valid || q->h_pin_valid || getenv("SG_NO_GPU_TOPK")) return 1;
+  if (P.nslots < (1u << 17) || getenv("SG_NO_GPU_TOPK")) return 1;
+  // a query holding a host copy answers from it: after the small-plan cross-GPU merge only that copy is merged, the
+  // device array is still this rank's own
+  if (q->acc.words) return 1;
   const unsigned cap = (unsigned)limit + 8192u;
   const size_t w = 2 + 2 * (size_t)naggs;
   const size_t off_tot = 0, off_hist = 512, off_offs = off_hist + 8192, off_scal = off_offs + 512, off_rows = off_scal + 128;
@@ -3399,51 +3513,23 @@ static int build_result_topk(sg_query* q, sg_result** out, bool* fell_back) {
   const unsigned long long* rows = (const unsigned long long*)(hp + off_rows);
   const uint64_t* scal = (const uint64_t*)(hp + off_scal);
 
-  // exact order of the candidates: value descending, ties by GroupByKey ascending (ranks of the rendered fields,
-  // or the keys themselves when the ranks do not give that order)
-  std::vector<std::vector<uint32_t>> scratch(q->dims.size());
-  std::vector<const std::vector<uint32_t>*> ranks(q->dims.size(), nullptr);
-  bool plain = true;
-  for (size_t di = 0; di < q->dims.size(); di++) ranks[di] = &axis_ranks(q, di, scratch[di], &plain);
-  struct Ent {
-    double v;
-    uint64_t tie;
-    uint32_t row;
-  };
-  std::vector<Ent> ents(n);
-  std::vector<std::string> keys(plain ? 0 : n);
+  // exact order of the candidates (keys rendered once each when the ranks do not give it)
+  GroupOrder O(q, true);
+  std::vector<GroupOrder::Ent> ents(n);
+  if (!O.plain) O.keys.resize(n);
   for (size_t i = 0; i < n; i++) {
     const unsigned long long* r = rows + i * w;
     const uint32_t sl = (uint32_t)r[0];
-    uint64_t tie = 0;
-    for (size_t di = 0; di < q->dims.size(); di++) {
-      const GroupDim& d = q->dims[di];
-      const uint32_t code = (sl / d.stride) % d.radix;
-      tie = tie * d.radix + (code ? (uint64_t)(*ranks[di])[code - 1] + 1u : 0u);
-    }
     ents[i].v = order_value(q, (int64_t)r[1], ob >= 0 ? (int64_t)r[2 + 2 * ob] : 0, ob >= 0 ? (int64_t)r[3 + 2 * ob] : 0);
-    ents[i].tie = tie;
+    ents[i].tie = O.tie(sl);
+    ents[i].slot = sl;
     ents[i].row = (uint32_t)i;
-    if (!plain) keys[i] = slot_key(q, sl);
+    if (!O.plain) O.keys[i] = slot_key(q, sl);
   }
-  std::sort(ents.begin(), ents.end(), [&](const Ent& a, const Ent& b) {
-    if (a.v != b.v) return a.v > b.v;
-    return plain ? a.tie < b.tie : keys[a.row] < keys[b.row];
-  });
+  std::sort(ents.begin(), ents.end(), [&](const GroupOrder::Ent& a, const GroupOrder::Ent& b) { return O.before(a, b); });
   if ((int64_t)ents.size() > limit) ents.resize((size_t)limit);
 
-  std::unique_ptr<sg_result> r(new sg_result());
-  r->q = q;
-  r->layouts = q->layouts;
-  r->hist_mode = false;
-  r->ngroups_cols = (int)q->groups.size();
-  r->naggs = naggs;
-  r->broken = q->broken_staged + (int64_t)scal[SC_BROKEN];
-  r->skipped = q->skipped;
-  init_group(r->total, naggs);
-  r->total.skey = "TOTAL";
-  for (int i = 1; i < (int)q->groups.size(); i++) r->total.skey += "\t";
-  r->has_total_hists = true;
+  std::unique_ptr<sg_result> r = new_result(q, false, scal);
   r->total.count = (int64_t)T.count;
   for (int a = 0; a < naggs; a++) {
     r->total.hc(a) = (int64_t)T.hc[a];
@@ -3525,27 +3611,24 @@ static void dense_fold(sg_query* q, const FoldKey& F, uint64_t* h, size_t have, 
 }
 
 // A folded sparse plan's read-back: the scalars and, of every accumulator region, the rows of the L' canonical
-// groups (ids 0..L'-1), into a pinned buffer the result owns, laid out for L' rows.  The query's layout becomes
-// that one (the next run lays the accumulators out again after its discovery).
-static int read_canonical_rows(sg_query* q, sg_result* r) {
+// groups (ids 0..L'-1), into a pinned buffer, laid out for L' rows.  The query's layout becomes that one (the next
+// run lays the accumulators out again after its discovery).
+static int read_canonical_rows(sg_query* q, HostAcc& h) {
   sg_ctx* c = q->ctx;
   const uint32_t n = q->canon_live;
   const std::vector<AccRegion> old = q->regions;
   int rc = layout_accumulators(q, n);
   if (rc != SG_OK) return rc;
   q->plan.nslots = n;
-  r->pin = c->pin_get(q->acc_words * 8, &r->pin_bytes);
-  if (!r->pin) {
-    c->set_err("cudaHostAlloc (result buffer) failed");
-    return SG_ERR_CUDA;
-  }
-  uint64_t* h = (uint64_t*)r->pin;
-  auto back = [&](size_t to, size_t from, size_t words) {
-    return words ? cudaMemcpyAsync(h + to, q->d_acc + from, words * 8, cudaMemcpyDeviceToHost, c->stream) : cudaSuccess;
-  };
-  CUDA_TRY(c, back(0, 0, SCALAR_WORDS));
-  for (size_t i = 0; i < old.size(); i++) CUDA_TRY(c, back(q->regions[i].off, old[i].off, (size_t)n * old[i].per_row));
-  CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+  rc = read_acc(q, h, q->acc_words, 0, nullptr, [&](uint64_t* dst) {
+    auto back = [&](size_t to, size_t from, size_t words) {
+      return words ? cudaMemcpyAsync(dst + to, q->d_acc + from, words * 8, cudaMemcpyDeviceToHost, c->stream) : cudaSuccess;
+    };
+    cudaError_t e = back(0, 0, SCALAR_WORDS);
+    for (size_t i = 0; i < old.size() && e == cudaSuccess; i++) e = back(q->regions[i].off, old[i].off, (size_t)n * old[i].per_row);
+    return e;
+  });
+  if (rc != SG_OK) return rc;
   q->d2h_bytes += (int64_t)q->acc_words * 8;
   return SG_OK;
 }
@@ -3574,41 +3657,23 @@ int build_result(sg_query* q, sg_result** out) {
   size_t have = q->acc_words;
   if (!want_max) have = q->sum_words;
   if (!want_max && !P.hist_mode && all_hc) have = q->prefix_words;
-  std::unique_ptr<sg_result> r(new sg_result());
-  r->q = q;
-  std::vector<uint64_t> hv;
-  const uint64_t* h = nullptr;
+  HostAcc acc;
   if (q->sparse && q->dfold) {
     // a folded sparse plan: the canonical groups hold ids 0..L'-1, and only their rows come back, laid out for L'
-    const int rc = read_canonical_rows(q, r.get());
+    const int rc = read_canonical_rows(q, acc);
     if (rc != SG_OK) return rc;
     have = q->acc_words;
-    h = (const uint64_t*)r->pin;
-  } else if (q->h_pin_valid && q->h_pin) {  // read back behind the kernel into a pinned buffer: the result takes it over
-    r->pin = q->h_pin;
-    r->pin_bytes = q->h_pin_bytes;
-    q->h_pin = nullptr;
-    q->h_pin_valid = false;
+  } else if (q->acc.words == q->acc_words) {  // read back behind the kernel or the merge: the result takes it over
+    acc = std::move(q->acc);
     have = q->acc_words;
-    h = (const uint64_t*)r->pin;
-  } else if (q->h_acc_valid && q->h_acc.size() == q->acc_words) {
-    hv.swap(q->h_acc);
-    q->h_acc_valid = false;
-    have = q->acc_words;
-    h = hv.data();
   } else {
-    // large results are read back into a pinned buffer the result keeps (a pageable destination is staged by
-    // the driver at a fraction of the PCIe rate, and a second copy would cost as much again)
-    r->pin = c->pin_get(have * 8, &r->pin_bytes);
-    if (!r->pin) {
-      c->set_err("cudaHostAlloc (result buffer) failed");
-      return SG_ERR_CUDA;
-    }
-    CUDA_TRY(c, cudaMemcpyAsync(r->pin, q->d_acc, have * 8, cudaMemcpyDeviceToHost, c->stream));
-    CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    const int rc = read_acc(q, acc, q->d_acc, have, 0, nullptr);
+    if (rc != SG_OK) return rc;
     q->d2h_bytes += (int64_t)have * 8;
-    h = (const uint64_t*)r->pin;
   }
+  std::unique_ptr<sg_result> r = new_result(q, P.hist_mode != 0, acc.data());
+  r->acc = std::move(acc);
+  uint64_t* const h = r->acc.data();  // (this result's own copy: the folds below change it)
   if (q->hashed) {
     if (h[SC_TABLE_FULL] != 0) {
       c->set_err("query: the hashed slot space filled up (more distinct group keys than its table holds)");
@@ -3646,7 +3711,7 @@ int build_result(sg_query* q, sg_result** out) {
     if (rc != SG_OK) return rc;
     F.wmul = wmul.data();
     F.luts = luts.data();
-    dense_fold(q, F, const_cast<uint64_t*>(h), have, r.get());  // (h is this call's own copy of the read-back)
+    dense_fold(q, F, h, have, r.get());
   }
   if (h[SC_NO_WEIGHT] != 0) {
     c->set_err(NO_WEIGHT_MSG);
@@ -3657,16 +3722,7 @@ int build_result(sg_query* q, sg_result** out) {
     w_rows = 0;
     for (uint64_t n : r->samples) w_rows += (int64_t)n;
   }
-  r->layouts = q->layouts;
-  r->hist_mode = P.hist_mode != 0;
-  r->ngroups_cols = (int)q->groups.size();
-  r->naggs = naggs;
   r->matched = (int64_t)h[SC_MATCHED];
-  r->broken = q->broken_staged + (int64_t)h[SC_BROKEN];
-  r->skipped = q->skipped;
-  init_group(r->total, naggs);
-  r->total.skey = "TOTAL";
-  for (int i = 1; i < (int)q->groups.size(); i++) r->total.skey += "\t";
   r->has_total_hists = !time_mode;
   const uint64_t* cnt = h + q->off_count;
   // a group is a slot that rows were scanned into.  Weighted, its Count is the sum of the rows' weights and can
@@ -3683,32 +3739,9 @@ int build_result(sg_query* q, sg_result** out) {
     int hw = (int)std::thread::hardware_concurrency();
     int nt = std::max(1, std::min(hw > 0 ? hw : 1, 16));
     if (const char* e = getenv("SG_HOST_THREADS")) nt = std::max(1, std::min(atoi(e), 16));  // tests: 1 vs many
-    // tie-break ranks: GroupByKey ascending == lexicographic over the axes' rendered fields, when `plain`;
-    // otherwise tied entries compare their rendered keys
-    std::vector<std::vector<uint32_t>> scratch(q->dims.size());
-    std::vector<const std::vector<uint32_t>*> ranks(q->dims.size(), nullptr);
-    bool plain = true;
-    if (ob != SG_ORDER_NONE)
-      for (size_t di = 0; di < q->dims.size(); di++) ranks[di] = &axis_ranks(q, di, scratch[di], &plain);
-    auto tie_of = [&](uint32_t s) {
-      uint64_t tie = 0;
-      const uint32_t cs = slot_code(q, s);
-      for (size_t di = 0; di < q->dims.size(); di++) {
-        const GroupDim& d = q->dims[di];
-        const uint32_t code = (cs / d.stride) % d.radix;
-        tie = tie * d.radix + (code ? (uint64_t)(*ranks[di])[code - 1] + 1u : 0u);
-      }
-      return tie;
-    };
-    struct Ent {
-      double v;
-      uint64_t tie;
-      uint32_t slot;
-    };
-    auto before = [&](const Ent& a, const Ent& b) {
-      if (a.v != b.v) return a.v > b.v;
-      return plain ? a.tie < b.tie : slot_key(q, a.slot) < slot_key(q, b.slot);
-    };
+    const GroupOrder O(q, ob != SG_ORDER_NONE);
+    using Ent = GroupOrder::Ent;
+    auto before = [&](const Ent& a, const Ent& b) { return O.before(a, b); };
     struct Part {
       std::vector<Ent> ents;
       ResultGroup tot;
@@ -3751,9 +3784,10 @@ int build_result(sg_query* q, sg_result** out) {
         }
         Ent e;
         e.slot = s;
+        e.row = 0;
         e.v = ob == SG_ORDER_NONE ? 0.0 : order_value(q, n, hc_o, sm_o);
         if (e.v < thr) continue;
-        e.tie = ob == SG_ORDER_NONE ? 0 : tie_of(s);
+        e.tie = ob == SG_ORDER_NONE ? 0 : O.tie(slot_code(q, s));
         p.ents.push_back(e);
         if (p.ents.size() >= trim_at) {
           std::nth_element(p.ents.begin(), p.ents.begin() + limit, p.ents.end(), before);
@@ -3772,20 +3806,7 @@ int build_result(sg_query* q, sg_result** out) {
     for (auto& p : parts) {
       live += p.live;
       all.insert(all.end(), p.ents.begin(), p.ents.end());
-      // Cumulative (aggregate.go:422-436): every group combined
-      r->total.count += p.tot.count;
-      for (int a = 0; a < naggs; a++) {
-        if (p.tot.hc(a) == 0) continue;
-        r->total.hc(a) += p.tot.hc(a);
-        r->total.sm(a) = (int64_t)((uint64_t)r->total.sm(a) + (uint64_t)p.tot.sm(a));
-        r->total.vx(a) = std::max(r->total.vx(a), p.tot.vx(a));
-        const uint32_t nv = q->layouts[(size_t)a].nvals_total;
-        if (nv && p.tot.values.size() > (size_t)a && !p.tot.values[(size_t)a].empty()) {
-          if (r->total.values.size() < (size_t)naggs) r->total.values.resize((size_t)naggs);
-          if (r->total.values[(size_t)a].empty()) r->total.values[(size_t)a].assign(nv, 0);
-          for (uint32_t k = 0; k < nv; k++) r->total.values[(size_t)a][k] += p.tot.values[(size_t)a][k];
-        }
-      }
+      merge_group(r->total, p.tot, naggs, q->layouts);  // Cumulative (aggregate.go:422-436): every group combined
     }
     if (ob != SG_ORDER_NONE) {
       std::sort(all.begin(), all.end(), before);
@@ -3800,15 +3821,8 @@ int build_result(sg_query* q, sg_result** out) {
     r->matched = w_rows >= 0 ? w_rows : r->total.count;
     if (w_rows >= 0) r->total.samples = w_rows;
     r->lazy = true;
-    r->acc_have = have;
     if (trace)
       fprintf(stderr, "sg_select: path=%s threads=%d\n", fell_back ? "device-fallback" : "host", ns >= (1u << 17) ? nt : 1);
-    if (!r->pin) {
-      r->acc.swap(hv);
-      r->accp = r->acc.data();
-    } else {
-      r->accp = h;
-    }
     *out = r.release();
     return SG_OK;
   }
@@ -3840,15 +3854,7 @@ int build_result(sg_query* q, sg_result** out) {
       r->total.samples = (r->total.samples < 0 ? 0 : r->total.samples) + g.samples;
     }
     auto& sl = slices[tbucket];
-    if (!sl) {
-      sl.reset(new sg_result());
-      sl->q = q;
-      sl->layouts = q->layouts;
-      sl->hist_mode = r->hist_mode;
-      sl->ngroups_cols = (int)q->groups.size();
-      sl->naggs = naggs;
-      init_group(sl->total, naggs);
-    }
+    if (!sl) sl = new_result(q, r->hist_mode, nullptr);
     sl->groups.push_back(std::move(g));
   }
   sort_groups(q, r->groups);
@@ -3918,7 +3924,6 @@ void sg_query_free(sg_query* q) {
   if (!q) return;
   cudaSetDevice(q->ctx->device);
   free_device(q);
-  if (q->h_pin) q->ctx->pin_put(q->h_pin, q->h_pin_bytes);
   if (q->ev0) cudaEventDestroy(q->ev0);
   if (q->ev1) cudaEventDestroy(q->ev1);
   if (q->ev2) cudaEventDestroy(q->ev2);
@@ -4102,7 +4107,7 @@ int sg_query_run(sg_query* q) {
     if (rc != SG_OK) return rc;
     rc = run_list(q, list);
     if (rc != SG_OK) return rc;
-    const uint64_t* scal = q->h_acc.data();  // read back behind the kernel by run_list
+    const uint64_t* scal = q->scal;  // read back behind the kernel by run_list
     if (scal[SC_TIME_OVERFLOW] != 0) {
       c->set_err("query: rows fall outside the planned time axis (time_min/time_max too narrow)");
       return SG_ERR_INVALID;
@@ -4419,8 +4424,7 @@ int sg_query_allreduce(sg_query* q) {
     c->set_err("allreduce: a hashed slot space (group-by product beyond 2^26) is merged on one GPU only in this build");
     return SG_ERR_UNSUPPORTED;
   }
-  q->h_acc_valid = false;  // the device copy is about to change
-  q->h_pin_valid = false;
+  q->acc.words = 0;  // the device copy is about to change
   // Small plans (the usual case: a few hundred groups): ONE collective.  Every rank writes a header
   // (block counters, signature of its axes) into its scalars and all-gathers its whole accumulator
   // array; each rank then reduces the gathered copies on the host (sum region, max region) — or, if
@@ -4462,8 +4466,7 @@ int sg_query_allreduce(sg_query* q) {
     for (size_t k = 0; k < nr; k++)
       for (int j = 0; j < 4; j++) tot[j] += all[k * aw + SC_MERGE + (size_t)j];
     if (agree) {
-      q->h_acc.assign(aw, 0);
-      uint64_t* h = q->h_acc.data();
+      uint64_t* h = q->acc.host(aw);  // build_result reads the merged host copy (the device copy stays per-rank)
       for (size_t w = 0; w < q->sum_words; w++) {
         uint64_t v = 0;
         for (size_t k = 0; k < nr; k++) v += all[k * aw + w];
@@ -4474,7 +4477,6 @@ int sg_query_allreduce(sg_query* q) {
         for (size_t k = 0; k < nr; k++) v = std::max(v, (int64_t)all[k * aw + w]);
         h[w] = (uint64_t)v;
       }
-      q->h_acc_valid = true;  // build_result reads the merged host copy (the device copy stays per-rank)
       q->broken_staged = (int64_t)tot[0];
       q->skipped = (int64_t)tot[1];
       q->rows_scanned = (int64_t)tot[2];
@@ -4530,21 +4532,6 @@ int sg_query_allreduce(sg_query* q) {
     hc[5] = sa * sa;
     hc[6] = sb;
     hc[7] = sb * sb;
-    uint64_t* hm = (uint64_t*)(hp + 64);
-    // a whole merged array of some size goes straight into a pinned buffer the result will own (no copy out of
-    // the scratch area afterwards: see run_list)
-    bool to_pin = false;
-    if (whole && q->acc_words * 8 >= ((size_t)32 << 10)) {
-      if (q->h_pin && q->h_pin_bytes < q->acc_words * 8) {
-        c->pin_put(q->h_pin, q->h_pin_bytes);
-        q->h_pin = nullptr;
-      }
-      if (!q->h_pin) q->h_pin = c->pin_get(q->acc_words * 8, &q->h_pin_bytes);
-      if (q->h_pin) {
-        hm = (uint64_t*)q->h_pin;
-        to_pin = true;
-      }
-    }
     cudaError_t ce = cudaMemcpyAsync(q->d_acc + SC_MERGE, hc, 64, cudaMemcpyHostToDevice, c->stream);
     if (ce == cudaSuccess) {
       rc = ar(q->d_acc, d_merged, q->sum_words, ncclUint64, ncclSum);
@@ -4552,9 +4539,17 @@ int sg_query_allreduce(sg_query* q) {
         rc = ar(q->d_acc + q->sum_words, d_merged + q->sum_words, q->acc_words - q->sum_words, ncclInt64, ncclMax);
     }
     if (ce == cudaSuccess && rc == SG_OK) ce = cudaMemsetAsync(q->d_acc + SC_MERGE, 0, 64, c->stream);  // own copy as it was
-    if (ce == cudaSuccess && rc == SG_OK)
-      ce = cudaMemcpyAsync(hm, d_merged, whole ? q->acc_words * 8 : 128, cudaMemcpyDeviceToHost, c->stream);
-    if (ce == cudaSuccess && rc == SG_OK) ce = cudaStreamSynchronize(c->stream);
+    // the merged array comes back whole into the query's host copy when small enough, else its scalars alone
+    uint64_t* hm = (uint64_t*)(hp + 64);
+    if (ce == cudaSuccess && rc == SG_OK) {
+      if (whole) {
+        rc = read_acc(q, q->acc, d_merged, q->acc_words, PIN_WHOLE_FROM, hp + 64);
+        hm = q->acc.data();
+      } else {
+        ce = cudaMemcpyAsync(hm, d_merged, 128, cudaMemcpyDeviceToHost, c->stream);
+        if (ce == cudaSuccess) ce = cudaStreamSynchronize(c->stream);
+      }
+    }
     if (ce != cudaSuccess || rc != SG_OK) {
       pool_release(c, d_merged);
       if (rc != SG_OK) return rc;
@@ -4574,22 +4569,17 @@ int sg_query_allreduce(sg_query* q) {
       if (ce == cudaSuccess && !whole) ce = cudaStreamSynchronize(c->stream);
       pool_release(c, d_merged);  // (stream-ordered pool: reuse waits for the copy queued above)
       if (ce != cudaSuccess) {
+        q->acc.words = 0;
         c->set_err(std::string("merge: ") + cudaGetErrorString(ce));
         return SG_ERR_CUDA;
       }
       if (whole) {
         for (int k = SC_MERGE; k < SCALAR_WORDS; k++) hm[k] = 0;
-        if (to_pin) {
-          q->h_acc.assign(hm, hm + SC_MERGE);
-          q->h_pin_valid = true;
-        } else {
-          q->h_acc.assign(hm, hm + q->acc_words);
-          q->h_acc_valid = true;
-        }
         q->d2h_bytes += (int64_t)q->acc_words * 8;
       }
       return SG_OK;
     }
+    q->acc.words = 0;  // (this rank's layout differs from others': the copy is no merge)
     pool_release(c, d_merged);
     rc = remap_to_union(q);  // differing dictionaries / time axes: re-lay this rank's accumulators by the union
     if (rc != SG_OK) return rc;
@@ -4627,15 +4617,13 @@ int sg_query_allreduce(sg_query* q) {
   if (rc == SG_OK && q->acc_words > q->sum_words)
     rc = ar(q->d_acc + q->sum_words, q->d_acc + q->sum_words, q->acc_words - q->sum_words, ncclInt64, ncclMax);
   if (rc != SG_OK) return rc;
-  // read the merged accumulators back behind the all-reduces (small plans): build_result then needs
-  // no further copy
+  // read the merged accumulators back behind the all-reduces (small plans, through the scratch area into a vector):
+  // build_result then needs no further copy
   if (whole) {
     char* hp = c->scratch(q->acc_words * 8);
     if (hp) {
-      CUDA_TRY(c, cudaMemcpyAsync(hp, q->d_acc, q->acc_words * 8, cudaMemcpyDeviceToHost, c->stream));
-      CUDA_TRY(c, cudaStreamSynchronize(c->stream));
-      q->h_acc.assign((const uint64_t*)hp, (const uint64_t*)hp + q->acc_words);
-      q->h_acc_valid = true;
+      rc = read_acc(q, q->acc, q->d_acc, q->acc_words, SIZE_MAX, hp);
+      if (rc != SG_OK) return rc;
       q->d2h_bytes += (int64_t)q->acc_words * 8;
       return SG_OK;
     }
@@ -4694,7 +4682,7 @@ static ResultGroup* pick_group(sg_result* r, int64_t i) {
     auto it = r->cache.find(i);
     if (it == r->cache.end()) {
       std::unique_ptr<ResultGroup> g(new ResultGroup());
-      make_group(r->q, r->accp, r->order[(size_t)i], *g, nullptr, r->samples.empty() ? nullptr : &r->samples);
+      make_group(r->q, r->acc.data(), r->order[(size_t)i], *g, nullptr, r->samples.empty() ? nullptr : &r->samples);
       it = r->cache.emplace(i, std::move(g)).first;
     }
     return it->second.get();
